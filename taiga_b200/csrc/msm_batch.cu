@@ -19,10 +19,13 @@
 //                           two-level weighted bucket reduction of msm.cu consumes.
 //
 // Exceptional pairs (equal points, opposite points, the identity) are handled inside the batch: their denominator is
-// replaced (2y for a doubling) or left out, so any input -- including the structured SRS of the tests -- is exact.
+// replaced (2y for a doubling) or left out, so any input -- including the structured SRS of the tests -- is exact.  The
+// forward kernel classifies every pair once and stores the kind beside the pair index; the backward kernel runs the plain
+// addition and sends the rare kinds to a cold branch.
 //
-// Algorithmic bytes: 64*N*W (table) + 32*N*K.  The rounds deliberately spend HBM bytes (each round writes its items) to
-// save integer instructions; DESIGN.md section 4 has the accounting.
+// The rounds spend HBM bytes (each round writes its items, ~330 B per pair addition) to save integer instructions; at the
+// shapes of the prover they stream ~2 TB/s, so their layout matters: items are stored as x / y planes, and round 0 keeps the
+// table indices of its pairs for the backward kernel.  DESIGN.md section 4.3 has the measured accounting.
 #define TB_NOINLINE_MUL 0   // every loop of this file is rolled (small code): inline multiplies keep live values in registers instead of spilling them around calls
 #include <cuda.h>
 #include <algorithm>
@@ -34,8 +37,7 @@
 namespace tb {
 
 constexpr int BA_THREADS = 256;
-constexpr int BA_M = 32;                        // default pairs per thread (TB_MSM_BA_M)
-constexpr int BA_PAIRS = BA_THREADS * BA_M;     // output items per CTA
+constexpr int BA_BWD_MINB = 3;                  // resident CTAs per SM of the backward kernel
 constexpr int BA_MAX_NB = 4096;
 constexpr int SORT_THREADS = 1024;
 constexpr int SORT_TILE = 1024;                 // scalars per pipeline stage (32 KB), one per thread
@@ -169,7 +171,10 @@ template <class F> __device__ __forceinline__ F lds_fe(const uint4* lo, const ui
   v.l[0] = x.x; v.l[1] = x.y; v.l[2] = x.z; v.l[3] = x.w; v.l[4] = y.x; v.l[5] = y.y; v.l[6] = y.z; v.l[7] = y.w; return v;
 }
 
-enum { PK_NONE = 0, PK_COPY1, PK_COPY2, PK_ADD, PK_DBL, PK_INF };
+// pair kinds, found once by the forward kernel and stored in the top bits of meta[q] = in0 | kind << META_KIND_SHIFT
+enum { PK_ADD = 0, PK_DBL, PK_COPY1, PK_COPY2, PK_INF };
+constexpr int META_KIND_SHIFT = 28;
+constexpr uint32_t META_IN0_MASK = (1u << META_KIND_SHIFT) - 1;
 
 // what a round needs to know about one MSM: the bucket offsets of its input (round r) and output (round r + 1) items
 struct RoundOffsets {
@@ -203,25 +208,23 @@ struct RoundOffsets {
 };
 constexpr size_t ba_off_bytes(int NB) { return (size_t)(2 * (NB + 4) + 32) * 4; }
 
-template <class B, bool FIRST> struct PairLoader {
-  const uint32_t* entries; const Aff<B>* table; const Aff<B>* items;
-  __device__ __forceinline__ Aff<B> point(uint32_t pos) const {
-    if (FIRST) {
-      const uint32_t e = __ldg(entries + pos);
-      Aff<B> p = ldg_aff(table + (e & 0x7fffffffu));
-      if (e >> 31) p.y = p.y.neg();
-      return p;
-    }
-    return ldg_aff(items + pos);
-  }
-  __device__ __forceinline__ B x(uint32_t pos) const {   // the identity is (0, 0): two identities give den = 0 and take the slow path
-    if (FIRST) return ldg_fe(&table[__ldg(entries + pos) & 0x7fffffffu].x);
-    return ldg_fe(&items[pos].x);
-  }
+// the items a round reads and writes, stored as two planes per MSM: x[0, cap) then y[0, cap).  The forward kernel reads the
+// x plane only, two adjacent coordinates per pair.
+template <class B> struct Planes {
+  B* x; long long cap;
+  __device__ __forceinline__ B ldx(uint32_t pos) const { return ldg_fe(x + pos); }
+  __device__ __forceinline__ Aff<B> ld(uint32_t pos) const { Aff<B> p; p.x = ldg_fe(x + pos); p.y = ldg_fe(x + cap + pos); return p; }
+  __device__ __forceinline__ void st(uint32_t pos, const Aff<B>& p) const { st_fe(x + pos, p.x); st_fe(x + cap + pos, p.y); }
 };
-// classification of a pair and its denominator; identical in the forward and the backward kernel
-template <class B> __device__ __forceinline__ int classify_pair(const Aff<B>& p1, const Aff<B>& p2, bool two, B& den) {
-  if (!two || p2.is_inf()) return PK_COPY1;
+// round 0 reads the window table through entries: e = (table index) | sign << 31
+template <class B> __device__ __forceinline__ Aff<B> table_point(const Aff<B>* table, uint32_t e) {
+  Aff<B> p = ldg_aff(table + (e & 0x7fffffffu));
+  if (e >> 31) p.y = p.y.neg();
+  return p;
+}
+// classification of a pair of two inputs whose x coordinates are equal or zero (the identity is (0, 0)), and its denominator
+template <class B> __device__ __forceinline__ int classify_pair(const Aff<B>& p1, const Aff<B>& p2, B& den) {
+  if (p2.is_inf()) return PK_COPY1;
   if (p1.is_inf()) return PK_COPY2;
   den = p2.x - p1.x;
   if (!den.is_zero()) return PK_ADD;
@@ -245,20 +248,25 @@ __global__ void __launch_bounds__(BA_THREADS) msm_ba_count_kernel(const uint32_t
   }
 }
 
-// ---- 2a. forward: prefix products of the denominators (to global memory), product tree of the CTA (to global memory)
-// A CTA owns BA_PAIRS consecutive output items of one MSM; thread t owns items Q0 + i * BA_THREADS + t.
+// ---- 2a. forward: classify every pair, prefix products of the denominators (to global memory), product tree of the CTA (to
+// global memory).  A CTA owns M * BA_THREADS consecutive output items of one MSM; thread t owns items Q0 + i * BA_THREADS + t.
+// Per item q it stores meta[q] = in0 | kind << META_KIND_SHIFT, and in round 0 the two signed table indices of the pair (eidx),
+// so that the backward kernel neither searches nor classifies again and gathers the table points without the entries load.
 template <class B, bool FIRST, int M>
 __global__ void __launch_bounds__(BA_THREADS) msm_ba_fwd_kernel(const uint32_t* __restrict__ counts0, int NB, int round, const uint32_t* __restrict__ entries,
-                                                                 const Aff<B>* __restrict__ table, const Aff<B>* __restrict__ items_in, long long cap_in, long long cap_out,
-                                                                 B* __restrict__ pre, B* __restrict__ tree, uint32_t* __restrict__ meta, const uint32_t* __restrict__ n_items, int R) {
+                                                                 const Aff<B>* __restrict__ table, const B* __restrict__ items_in, long long cap_in, long long cap_out,
+                                                                 B* __restrict__ pre, B* __restrict__ tree, uint32_t* __restrict__ meta, uint2* __restrict__ eidx,
+                                                                 const uint32_t* __restrict__ n_items, int R) {
   extern __shared__ __align__(16) uint8_t ba_smem[];
   const int k = blockIdx.y, t = threadIdx.x;
   const uint32_t Q0 = blockIdx.x * (M * BA_THREADS);
   if (Q0 >= n_items[(long long)k * (R + 1) + round + 1]) return;   // nothing of this MSM left for this CTA (uniform over the CTA)
   RoundOffsets ro; ro.build(ba_smem, counts0 + (long long)k * NB, NB, round);
-  PairLoader<B, FIRST> ld{entries + (FIRST ? (long long)k * cap_in : 0), table, items_in + (FIRST ? 0 : (long long)k * cap_in)};
-  B* pre_k = pre + (long long)k * cap_out;
+  const uint32_t* ent_k = entries + (long long)k * cap_in;
+  const Planes<B> in{const_cast<B*>(items_in) + 2 * (long long)k * cap_in, cap_in};
+  B* pre_k = pre + 2 * (long long)k * cap_out;   // the y plane of this round's output (see msm_batch_buckets)
   uint32_t* meta_k = meta + (long long)k * cap_out;
+  uint2* eidx_k = eidx + (long long)k * cap_out;
   B acc = B::one();
   int hint = 0;
 #pragma unroll 1
@@ -266,17 +274,21 @@ __global__ void __launch_bounds__(BA_THREADS) msm_ba_fwd_kernel(const uint32_t* 
     const uint32_t q = Q0 + (uint32_t)i * BA_THREADS + t;
     if (q >= ro.n_next) break;
     uint32_t in0; bool two; ro.locate(q, NB, in0, two, hint);
-    meta_k[q] = in0 | (two ? 0x80000000u : 0u);   // the backward kernel does not search again
     st_fe(pre_k + q, acc);
-    if (!two) continue;
-    const B x1 = ld.x(in0), x2 = ld.x(in0 + 1);    // the common case needs the x coordinates only
-    B den = x2 - x1;
-    if (den.is_zero() || x1.is_zero() || x2.is_zero()) {   // equal x (doubling / cancellation) or possibly an identity (0, 0): classify on the full points
-      const Aff<B> p1 = ld.point(in0), p2 = ld.point(in0 + 1);
-      const int kind = classify_pair(p1, p2, two, den);
-      if (kind != PK_ADD && kind != PK_DBL) continue;
+    int kind = PK_COPY1;
+    uint2 e = make_uint2(0, 0);
+    if (FIRST) { e.x = __ldg(ent_k + in0); if (two) e.y = __ldg(ent_k + in0 + 1); eidx_k[q] = e; }
+    if (two) {
+      const B x1 = FIRST ? ldg_fe(&table[e.x & 0x7fffffffu].x) : in.ldx(in0), x2 = FIRST ? ldg_fe(&table[e.y & 0x7fffffffu].x) : in.ldx(in0 + 1);
+      B den = x2 - x1;
+      kind = PK_ADD;
+      if (den.is_zero() || x1.is_zero() || x2.is_zero()) {   // equal x (doubling / cancellation) or possibly an identity (0, 0): classify on the full points
+        const Aff<B> p1 = FIRST ? table_point(table, e.x) : in.ld(in0), p2 = FIRST ? table_point(table, e.y) : in.ld(in0 + 1);
+        kind = classify_pair(p1, p2, den);
+      }
+      if (kind == PK_ADD || kind == PK_DBL) acc = acc * den;
     }
-    acc = acc * den;
+    meta_k[q] = in0 | (uint32_t)kind << META_KIND_SHIFT;
   }
   __syncthreads();   // the offset arrays are dead: the product tree (heap layout, nd[1] = root, leaves nd[BA_THREADS + t]) takes their place
   B* nd = reinterpret_cast<B*>(ba_smem);
@@ -299,12 +311,12 @@ __global__ void msm_ba_inv_kernel(B* __restrict__ tree, uint32_t n_trees) {
   st_fe(root, ld_fe(root).inv());
 }
 
-// ---- 2c. backward: push the inverted root down the tree, then walk every thread's pairs back and write the sums
-template <class B, bool FIRST, int M, int MINB>
-__global__ void __launch_bounds__(BA_THREADS, MINB) msm_ba_bwd_kernel(const uint32_t* __restrict__ counts0, int NB, int round, const uint32_t* __restrict__ entries,
-                                                                 const Aff<B>* __restrict__ table, const Aff<B>* __restrict__ items_in, long long cap_in,
-                                                                 Aff<B>* __restrict__ items_out, long long cap_out, const B* __restrict__ pre, const B* __restrict__ tree,
-                                                                 const uint32_t* __restrict__ meta, const uint32_t* __restrict__ n_items, int R) {
+// ---- 2c. backward: push the inverted root down the tree, then walk every thread's pairs back and write the sums.
+// BA_BWD_MINB resident CTAs per SM (80 registers): faster on H100 than 2 (more registers, fewer warps) or 4 (64 registers, spills).
+template <class B, bool FIRST, int M>
+__global__ void __launch_bounds__(BA_THREADS, BA_BWD_MINB) msm_ba_bwd_kernel(const Aff<B>* __restrict__ table, const B* __restrict__ items_in, long long cap_in,
+                                                                 B* __restrict__ items_out, long long cap_out, const B* __restrict__ tree,
+                                                                 const uint32_t* __restrict__ meta, const uint2* __restrict__ eidx, const uint32_t* __restrict__ n_items, int round, int R) {
   extern __shared__ __align__(16) uint8_t ba_smem[];
   const int k = blockIdx.y, t = threadIdx.x;
   const uint32_t Q0 = blockIdx.x * (M * BA_THREADS);
@@ -323,43 +335,44 @@ __global__ void __launch_bounds__(BA_THREADS, MINB) msm_ba_bwd_kernel(const uint
     __syncthreads();
   }
   B inv_run = nd[BA_THREADS + t];   // 1 / (product of this thread's denominators)
-  PairLoader<B, FIRST> ld{entries + (FIRST ? (long long)k * cap_in : 0), table, items_in + (FIRST ? 0 : (long long)k * cap_in)};
-  const B* pre_k = pre + (long long)k * cap_out;
+  const Planes<B> in{const_cast<B*>(items_in) + 2 * (long long)k * cap_in, cap_in}, out{items_out + 2 * (long long)k * cap_out, cap_out};
   const uint32_t* meta_k = meta + (long long)k * cap_out;
-  Aff<B>* out = items_out + (long long)k * cap_out;
+  const uint2* eidx_k = eidx + (long long)k * cap_out;
+  // the prefix products of the forward kernel sit in the y plane of the output: slot q is read (plain, coherent load) by this
+  // thread before it writes out.y[q] over it
+  const B* pre_k = out.x + cap_out;
   int last = M - 1;
   while (last >= 0 && Q0 + (uint32_t)last * BA_THREADS + t >= n_next) --last;
 #pragma unroll 1
   for (int i = last; i >= 0; --i) {
     const uint32_t q = Q0 + (uint32_t)i * BA_THREADS + t;
     const uint32_t mt = __ldg(meta_k + q);
-    const uint32_t in0 = mt & 0x7fffffffu; const bool two = mt >> 31;
-    const Aff<B> p1 = ld.point(in0);
-    Aff<B> p2 = p1;
-    if (two) p2 = ld.point(in0 + 1);
-    B den;
-    const int kind = classify_pair(p1, p2, two, den);
+    const uint2 e = FIRST ? __ldg(eidx_k + q) : make_uint2(0, 0);   // round 0: loaded beside meta, one load before the table gather
+    const uint32_t in0 = mt & META_IN0_MASK, kind = mt >> META_KIND_SHIFT;
+    const Aff<B> p1 = FIRST ? table_point(table, e.x) : in.ld(in0);
     Aff<B> r;
-    if (kind == PK_COPY1) r = p1;
-    else if (kind == PK_COPY2) r = p2;
-    else if (kind == PK_INF) r = Aff<B>::inf();
-    else {
-      const B dinv = inv_run * ldg_fe(pre_k + q);   // 1 / den
+    if (kind <= PK_DBL) {   // an addition (the common case) or, rarely, a doubling: lambda = num / den
+      Aff<B> p2 = p1;
+      B num, den;
+      if (kind == PK_ADD) { p2 = FIRST ? table_point(table, e.y) : in.ld(in0 + 1); num = p2.y - p1.y; den = p2.x - p1.x; }
+      else { const B x2 = p1.x.sqr(); num = x2.dbl() + x2; den = p1.y.dbl(); }
+      const B dinv = inv_run * ld_fe(pre_k + q);   // 1 / den
       inv_run = inv_run * den;
-      B num;
-      if (kind == PK_ADD) num = p2.y - p1.y;
-      else { const B x2 = p1.x.sqr(); num = x2.dbl() + x2; }
       const B lam = num * dinv;
       r.x = lam.sqr() - p1.x - p2.x;
       r.y = lam * (p1.x - r.x) - p1.y;
+    } else {   // rare: the identity, a pair that cancels, a bucket's odd item out
+      r = p1;
+      if (kind == PK_COPY2) r = FIRST ? table_point(table, e.y) : in.ld(in0 + 1);
+      else if (kind == PK_INF) r = Aff<B>::inf();
     }
-    st_fe(&out[q].x, r.x); st_fe(&out[q].y, r.y);
+    out.st(q, r);
   }
 }
 
 // ---------------------------------------------------------------- 3. what is left in every bucket -> XYZZ bucket sums
 template <class B>
-__global__ void __launch_bounds__(BA_THREADS) msm_ba_finish_kernel(const uint32_t* __restrict__ counts0, int NB, int round, const Aff<B>* __restrict__ items, long long cap,
+__global__ void __launch_bounds__(BA_THREADS) msm_ba_finish_kernel(const uint32_t* __restrict__ counts0, int NB, int round, const B* __restrict__ items, long long cap,
                                                                     Xyzz<B>* __restrict__ buckets) {
   extern __shared__ __align__(16) uint8_t fin_smem[];
   uint32_t* off = reinterpret_cast<uint32_t*>(fin_smem);   // [NB + 1]
@@ -371,8 +384,8 @@ __global__ void __launch_bounds__(BA_THREADS) msm_ba_finish_kernel(const uint32_
   const int b = blockIdx.x * BA_THREADS + t;
   if (b >= NB) return;
   Xyzz<B> acc = Xyzz<B>::inf();
-  const Aff<B>* it = items + (long long)k * cap;
-  for (uint32_t p = off[b]; p < off[b + 1]; ++p) acc.add_affine(ldg_aff(it + p));
+  const Planes<B> it{const_cast<B*>(items) + 2 * (long long)k * cap, cap};
+  for (uint32_t p = off[b]; p < off[b + 1]; ++p) acc.add_affine(it.ld(p));
   buckets[(long long)k * NB + b] = acc;
 }
 
@@ -390,23 +403,21 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// one reduction round = forward, root inversion, backward; (pairs per thread, resident CTAs per SM) are tuning parameters
-template <class B, bool FIRST, int M, int MINB>
-static void launch_round_t(Ctx* ctx, dim3 grid, size_t fwd_smem, size_t bwd_smem, const uint32_t* counts, int NB, int r, const uint32_t* entries, const Aff<B>* table, const Aff<B>* in,
-                           long long cap_in, Aff<B>* out, long long cap_out, B* pre, B* tree, uint32_t* meta, const uint32_t* n_items, int R, uint32_t n_trees) {
+// one reduction round = forward, root inversion, backward; M (pairs per thread) is a tuning parameter: 32 is faster on dense
+// scalars, 16 on sparse witness columns (more CTAs share out the few pairs of the later rounds)
+template <class B, bool FIRST, int M>
+static void launch_round_t(Ctx* ctx, dim3 grid, size_t fwd_smem, size_t bwd_smem, const uint32_t* counts, int NB, int r, const uint32_t* entries, const Aff<B>* table, const B* in,
+                           long long cap_in, B* out, long long cap_out, B* pre, B* tree, uint32_t* meta, uint2* eidx, const uint32_t* n_items, int R, uint32_t n_trees) {
   cudaStream_t st = ctx->stream;
   ctx->opt_in_smem(msm_ba_fwd_kernel<B, FIRST, M>, fwd_smem);
-  ctx->opt_in_smem(msm_ba_bwd_kernel<B, FIRST, M, MINB>, bwd_smem);
-  msm_ba_fwd_kernel<B, FIRST, M><<<grid, BA_THREADS, fwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, n_items, R);
+  ctx->opt_in_smem(msm_ba_bwd_kernel<B, FIRST, M>, bwd_smem);
+  msm_ba_fwd_kernel<B, FIRST, M><<<grid, BA_THREADS, fwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, eidx, n_items, R);
   msm_ba_inv_kernel<B><<<(n_trees + 63) / 64, 64, 0, st>>>(tree, n_trees);
-  msm_ba_bwd_kernel<B, FIRST, M, MINB><<<grid, BA_THREADS, bwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, out, cap_out, pre, tree, meta, n_items, R);
+  msm_ba_bwd_kernel<B, FIRST, M><<<grid, BA_THREADS, bwd_smem, st>>>(table, in, cap_in, out, cap_out, tree, meta, eidx, n_items, r, R);
 }
-template <class B, typename... A> static void launch_round(Ctx* ctx, int M, int minb, bool first, A... a) {
-#define TB_LR(MM, NN) (first ? launch_round_t<B, true, MM, NN>(ctx, a...) : launch_round_t<B, false, MM, NN>(ctx, a...))
-  if (M == 8) { if (minb == 2) TB_LR(8, 2); else if (minb == 3) TB_LR(8, 3); else TB_LR(8, 4); }
-  else if (M == 32) { if (minb == 2) TB_LR(32, 2); else if (minb == 3) TB_LR(32, 3); else TB_LR(32, 4); }
-  else { if (minb == 2) TB_LR(16, 2); else if (minb == 3) TB_LR(16, 3); else TB_LR(16, 4); }
-#undef TB_LR
+template <class B, typename... A> static void launch_round(Ctx* ctx, int M, bool first, A... a) {
+  if (M == 32) { if (first) launch_round_t<B, true, 32>(ctx, a...); else launch_round_t<B, false, 32>(ctx, a...); }
+  else { if (first) launch_round_t<B, true, 16>(ctx, a...); else launch_round_t<B, false, 16>(ctx, a...); }
 }
 
 bool msm_batch_applicable(int N, int K, const MsmConfig& cfg, int c) {
@@ -427,12 +438,18 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
   const int R = tb_tune("TB_MSM_BA_ROUNDS", 10);
   TB_REQUIRE(R >= 1 && R <= 20, "TB_MSM_BA_ROUNDS out of range");
   for (int r = 0; r < R; ++r) cap.push_back((cap.back() + NB + 1) / 2);
-  // MSMs per chunk: one wave of the sort kernel (one 1024-thread CTA per SM).  A chunk's temporaries take ~47 MB per MSM
-  // from the stream-ordered pool, which keeps them cached: ~6 GB per proving stream on H100 at this size.
+  TB_REQUIRE(cap0 <= (long long)META_IN0_MASK + 1, "too many MSM entries for the pair index of meta");
+  // MSMs per chunk: one wave of the sort kernel (one 1024-thread CTA per SM).  A chunk's temporaries take ~36 MB per MSM
+  // from the stream-ordered pool, which keeps them cached: ~4.8 GB per proving stream on H100 at this size.
   const int Kc_max = tb_tune("TB_MSM_BA_CHUNK", ctx->sm_count);
   const int Kc = K < Kc_max ? K : Kc_max;
   DevBuf<uint32_t> counts(ctx, (size_t)Kc * NB), entries(ctx, (size_t)Kc * cap0);
-  DevBuf<Aff<B>> itA(ctx, (size_t)Kc * cap[1]), itB(ctx, (size_t)Kc * (R > 1 ? cap[2] : 1));
+  // round items as x / y planes (2 * cap field elements per MSM).  The prefix products of a round live in the y plane of its
+  // output until the backward kernel overwrites them (each slot is read, then written, by the same thread).  itB is free
+  // during round 0 and holds its table indices (8 B per output item, a quarter of a field element).
+  const size_t eidx_fe = ((size_t)Kc * cap[1] + 3) / 4;
+  DevBuf<B> itA(ctx, (size_t)Kc * 2 * cap[1]), itB(ctx, std::max(R > 1 ? (size_t)(Kc * 2 * cap[2]) : (size_t)0, eidx_fe));
+  uint2* eidx = reinterpret_cast<uint2*>(itB.get());
   const size_t sort_smem = 2 * SORT_TILE * sizeof(S) + 16 + (size_t)(NB + 1 + 32) * 4 + 16;
   const size_t fwd_smem = std::max(ba_off_bytes(NB), (size_t)2 * BA_THREADS * sizeof(B));
   const size_t bwd_smem = (size_t)2 * BA_THREADS * sizeof(B);
@@ -440,10 +457,10 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
   ctx->opt_in_smem(msm_sort_kernel<S, 13>, sort_smem);
   ctx->opt_in_smem(msm_sort_kernel<S, 0>, sort_smem);
   ctx->opt_in_smem(msm_ba_finish_kernel<B>, fin_smem);
-  const int Mv = tb_tune("TB_MSM_BA_M", 32) >= 32 ? 32 : tb_tune("TB_MSM_BA_M", 32) <= 8 ? 8 : 16, minb = tb_tune("TB_MSM_BA_MINB", 3) <= 2 ? 2 : tb_tune("TB_MSM_BA_MINB", 3) >= 4 ? 4 : 3;
+  const int Mv = tb_tune("TB_MSM_BA_M", 32) >= 32 ? 32 : 16;
   const long long pairs_per_cta = (long long)Mv * BA_THREADS;
   const unsigned ctas1 = (unsigned)((cap[1] + pairs_per_cta - 1) / pairs_per_cta);
-  DevBuf<B> pre(ctx, (size_t)Kc * cap[1]), tree(ctx, (size_t)Kc * ctas1 * 2 * BA_THREADS);
+  DevBuf<B> tree(ctx, (size_t)Kc * ctas1 * 2 * BA_THREADS);
   DevBuf<uint32_t> meta(ctx, (size_t)Kc * cap[1]), n_items(ctx, (size_t)Kc * (R + 1));
   for (int k0 = 0; k0 < K; k0 += Kc) {
     const int kc = K - k0 < Kc ? K - k0 : Kc;
@@ -463,16 +480,16 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
     { ProfScope ps(ctx, PC_MSM_ACCUM);
       msm_ba_count_kernel<<<kc, BA_THREADS, 0, st>>>(counts.get(), NB, R, n_items.get());
       for (int r = 0; r < R; ++r) {
-        const Aff<B>* in = (r & 1) ? itA.get() : itB.get();   // round r reads what round r-1 wrote (r = 0 reads the entries)
-        Aff<B>* out = (r & 1) ? itB.get() : itA.get();
+        const B* in = (r & 1) ? itA.get() : itB.get();   // round r reads what round r-1 wrote (r = 0 reads the entries)
+        B* out = (r & 1) ? itB.get() : itA.get();
         const unsigned gx = (unsigned)((cap[r + 1] + pairs_per_cta - 1) / pairs_per_cta);
         dim3 grid(gx, kc);
         const uint32_t n_trees = gx * (uint32_t)kc;
-        launch_round<B>(ctx, Mv, minb, r == 0, grid, fwd_smem, bwd_smem, counts.get(), NB, r, entries.get(), table, in, r == 0 ? cap0 : cap[r], out, cap[r + 1], pre.get(), tree.get(),
-                        meta.get(), n_items.get(), R, n_trees);
+        launch_round<B>(ctx, Mv, r == 0, grid, fwd_smem, bwd_smem, counts.get(), NB, r, entries.get(), table, in, r == 0 ? cap0 : cap[r], out, cap[r + 1], out + cap[r + 1], tree.get(),
+                        meta.get(), eidx, n_items.get(), R, n_trees);
         TB_LAUNCH_CHECK(); ctx->launches += 3;
       }
-      const Aff<B>* last = (R & 1) ? itA.get() : itB.get();
+      const B* last = (R & 1) ? itA.get() : itB.get();
       msm_ba_finish_kernel<B><<<dim3((NB + BA_THREADS - 1) / BA_THREADS, kc), BA_THREADS, fin_smem, st>>>(counts.get(), NB, R, last, cap[R], buckets + (size_t)k0 * NB);
       TB_LAUNCH_CHECK(); ctx->launches++; }
   }
