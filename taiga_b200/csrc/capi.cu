@@ -126,7 +126,7 @@ static void dev_msm(Ctx* c, size_t n, uint32_t batch, const S* scalars, const Af
   DevBuf<Xyzz<B>> acc(c, batch);
   MsmConfig cfg; cfg.c = (int)window_bits;
   msm_run<B, S>(c, scalars, (long long)n, points, 0, (int)n, (int)batch, cfg, acc.get());
-  points_finalize<B, S>(c, acc.get(), (int)batch, nullptr, nullptr, 0, out);
+  points_to_affine<B>(c, acc.get(), (int)batch, out);
 }
 
 template <class B, class S>

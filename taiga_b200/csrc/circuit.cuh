@@ -25,17 +25,19 @@ struct Circuit {
   uint32_t k, na, nf, ni, degree, bf, P, L, chunk, nsets, pieces; int ext_k, R; size_t n, usable;
   std::vector<tb_query> aq, fq, iq; std::vector<tb_column> perm;
   std::vector<tb_expr_node> nodes; std::vector<uint32_t> roots; std::vector<uint8_t> consts_bytes; uint32_t nconsts;
-  std::vector<std::vector<uint32_t>> lk_in, lk_tab; std::vector<tb_lookup> lk_desc;
+  std::vector<std::vector<uint32_t>> lk_in, lk_tab;
   Fp vk_repr;  // canonical
   // device tables
   Fp *fixed_vals = nullptr, *fixed_polys = nullptr, *fixed_cosets = nullptr, *sig_vals = nullptr, *sig_polys = nullptr, *sig_cosets = nullptr;
   Fp *l0 = nullptr, *l_last = nullptr, *l_blind = nullptr, *consts = nullptr, *wr_inv = nullptr;
   Fp* coset_pre = nullptr;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
-  int2 *d_aq = nullptr, *d_fq = nullptr, *d_iq = nullptr, *d_perm = nullptr;
+  int2* d_perm = nullptr;
   QProgram prog_lookups;
-  // gate programs keyed by number of parts: `gate_parts` holds the constraints evaluated on every sub-coset (all of them when the
+  // gate programs in gate_nparts[big] parts, big = (batch size >= 8): small batches run more, shorter programs (latency), large
+  // ones fewer (less duplicated work).  `gate_parts` holds the constraints evaluated on every sub-coset (all of them when the
   // circuit is not split), `gate_parts_lo` the low-degree ones (degree <= R / 2) that are evaluated on every second sub-coset only
-  std::map<int, std::vector<QProgram>> gate_parts, gate_parts_lo;
+  static constexpr int gate_nparts[2] = {8, 4};
+  std::vector<QProgram> gate_parts[2], gate_parts_lo[2];
   bool split = false; uint32_t num_constraints = 0, t_pl = 0;   // t_pl: permutation + lookup terms folded after the gates
   std::vector<Fp> t_inv; Fp delta, zeta, omega, r_inv;
   Fp delta_c0[16];
@@ -78,10 +80,10 @@ struct Circuit {
   ~Circuit() {
     for (auto& kv : ws) { for (auto& b : kv.second->blocks) cudaFree(b.p); for (void* p : kv.second->tables) cudaFree(p); }
     for (void* p : {(void*)fixed_vals, (void*)fixed_polys, (void*)fixed_cosets, (void*)sig_vals, (void*)sig_polys, (void*)sig_cosets, (void*)l0, (void*)l_last,
-                    (void*)l_blind, (void*)consts, (void*)wr_inv, (void*)coset_pre, (void*)d_aq, (void*)d_fq, (void*)d_iq, (void*)d_perm, (void*)prog_lookups.dev})
+                    (void*)l_blind, (void*)consts, (void*)wr_inv, (void*)coset_pre, (void*)d_perm, (void*)prog_lookups.dev})
       if (p) cudaFree(p);
-    for (auto& kv : gate_parts) for (auto& qp : kv.second) if (qp.dev) cudaFree(qp.dev);
-    for (auto& kv : gate_parts_lo) for (auto& qp : kv.second) if (qp.dev) cudaFree(qp.dev);
+    for (auto& progs : gate_parts) for (auto& qp : progs) if (qp.dev) cudaFree(qp.dev);
+    for (auto& progs : gate_parts_lo) for (auto& qp : progs) if (qp.dev) cudaFree(qp.dev);
   }
 };
 

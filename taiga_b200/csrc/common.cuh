@@ -43,7 +43,10 @@ enum ProfCat { PC_NTT = 0, PC_MSM_SORT, PC_MSM_ACCUM, PC_MSM_REDUCE, PC_QUOT_GAT
                PC_POLY, PC_COUNT };
 struct ProfRec { int cat; cudaEvent_t a, b; };
 
-// experiment knob: integer from the environment (read on every call; only used on host set-up paths)
+// Integer from the environment (read on every call; only on host set-up paths).  A variable is read only if a test sets it
+// to compare two shipped paths on the same input, or to reach a shipped path that the test's inputs would not reach:
+// TB_MSM_BA_MIN_TERMS, TB_MSM_BA_ROUNDS, TB_MSM_BA_CHUNK (msm_batch.cu), TB_Q_SPLIT (prover.cu); TB_DEBUG prints the
+// quotient's degree split at circuit load.  Every other launch choice is a constant of the code.
 inline int tb_tune(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 
 struct Ctx {

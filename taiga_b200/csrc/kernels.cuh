@@ -23,14 +23,13 @@ template <class F> void free_twiddles(Ctx* ctx);
 
 // ---------------------------------------------------------------- MSM (msm.cu)
 struct MsmConfig {
-  int c = 0;             // window bits (0 = choose from N)
+  int c = 0;             // window bits (0 = choose from N; a fixed-base table needs the c it was built with)
   int table_windows = 0;  // >0: `bases` is a fixed-base table [table_windows][table_stride] of 2^(c*w)*B_i and all windows share one bucket set
   int table_stride = 0;   // points per table window (>= N + n_extra); 0 = N
   int n_extra = 0;        // extra terms per MSM: scalar extra_scalars[k*n_extra + j] (Montgomery) times table point N + j
   const void* extra_scalars = nullptr;
   void* affine_out = nullptr;  // fixed-base mode: also write the K results normalised to affine (Aff<B>[K])
 };
-int msm_default_window(int n, bool fixed_tables);
 // K multi-scalar multiplications of N terms.  scalars: Montgomery form, item k at scalars + k*scalar_bstride.
 // bases: affine Montgomery; item k at bases + k*base_bstride (0 = shared).  out: K XYZZ points.
 template <class B, class S>
@@ -44,9 +43,6 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
 // table[w][i] = 2^(c*w) * bases[i], w < windows  (one-off, at SRS load)
 template <class B> void msm_build_tables(Ctx* ctx, const Aff<B>* bases, int N, int c, int windows, Aff<B>* table);
 template <class B> void points_to_affine(Ctx* ctx, const Xyzz<B>* acc, int K, Aff<B>* out);
-// out[k] = affine(acc[k] + sum_j extra_scalars[k*n_extra+j] * extra_bases[j]); scalars Montgomery
-template <class B, class S>
-void points_finalize(Ctx* ctx, const Xyzz<B>* acc, int K, const S* extra_scalars, const Aff<B>* extra_bases, int n_extra, Aff<B>* out);
 
 // ---------------------------------------------------------------- elementwise helpers (poly.cu)
 template <class F> void fe_to_mont(Ctx* ctx, F* v, size_t n);     // canonical -> Montgomery, in place

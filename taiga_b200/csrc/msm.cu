@@ -18,12 +18,13 @@
 namespace tb {
 
 constexpr int MSM_CHUNK_MAX = 64;  // max entries accumulated by one thread (adaptive: chosen so the accumulation fills the GPU)
+constexpr int MSM_UNITS_PER_SM = 2048;       // accumulation units aimed at per SM when choosing the chunk
+constexpr int MSM_SUB_WARPS_PER_SM = 16;     // warps per SM the sub-warp combine aims at when choosing its lanes per bucket
 constexpr int MSM_SEG = 8;         // buckets per thread in the running-sum reduction
-constexpr int MSM_FIXED_C = 13;    // fixed-base window: 4096 buckets per MSM, 20 table windows (measured best of 11/12/13/16 at k = 15)
 constexpr uint32_t MSM_HEAVY_UNITS = 1024;  // buckets with more units than this get a whole CTA (e.g. the top window of a variable-base MSM)
 
-int msm_default_window(int n, bool fixed_tables) {
-  if (fixed_tables) return MSM_FIXED_C;
+// variable-base window from the MSM length (fixed-base callers pass the c their tables were built with)
+static int msm_default_window(int n) {
   int lg = 0; while ((1 << (lg + 1)) <= n) ++lg;
   int c = lg - 4;
   if (c < 4) c = 4;
@@ -79,8 +80,8 @@ __global__ void msm_units_kernel(const uint32_t* __restrict__ offs, uint32_t nb_
   else if (uc > sub_units) mid[atomicAdd(n_lists, 1u)] = b;
 }
 
-template <class B, int MINB>
-__global__ void __launch_bounds__(128, MINB) msm_accum_kernel(const Aff<B>* __restrict__ bases, long long base_bstride, uint32_t buckets_per_item,
+template <class B>
+__global__ void __launch_bounds__(128, 4) msm_accum_kernel(const Aff<B>* __restrict__ bases, long long base_bstride, uint32_t buckets_per_item,
                                  const uint32_t* __restrict__ offs, const uint32_t* __restrict__ unit_off, uint32_t nb_total, uint32_t chunk,
                                  const uint32_t* __restrict__ entries, Xyzz<B>* __restrict__ partial) {
   uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
@@ -322,7 +323,7 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
              const MsmConfig& cfg_in, Xyzz<B>* out) {
   TB_REQUIRE(N >= 1 && K >= 1 && K <= 65535, "MSM shape out of range");
   const bool table_mode = cfg_in.table_windows > 0;
-  int c = cfg_in.c ? cfg_in.c : msm_default_window(N, table_mode);
+  int c = cfg_in.c ? cfg_in.c : msm_default_window(N);
   TB_REQUIRE(c >= 2 && c <= 20, "MSM window out of range");
   const int W = (256 + c - 1) / c;
   if (table_mode) TB_REQUIRE(cfg_in.table_windows >= W, "fixed-base table has too few windows");
@@ -359,7 +360,7 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
 
     // adaptive chunk: aim at ~4 waves of 512 threads per SM so that small batches still fill the machine
     uint32_t chunk_log = 3;
-    { const uint64_t target_units = (uint64_t)tb_tune("TB_MSM_UNITS_PER_SM", 2048) * (uint64_t)ctx->sm_count;
+    { const uint64_t target_units = (uint64_t)MSM_UNITS_PER_SM * (uint64_t)ctx->sm_count;
       while ((1u << chunk_log) < (uint32_t)MSM_CHUNK_MAX && (max_entries >> chunk_log) > target_units) ++chunk_log; }
     const uint64_t max_units = nb_total64 + (max_entries >> chunk_log) + 1;
     const uint64_t max_heavy = (max_entries >> chunk_log) / MSM_HEAVY_UNITS + 1;
@@ -367,7 +368,7 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
     // CTA each).  lanes: as wide as keeps ~4 warps per SM sub-partition busy, no wider than the average bucket needs.
     uint32_t lpb_log = 0;
     { const uint64_t avg_units = ((max_entries >> chunk_log) + nb_total64 - 1) / nb_total64;
-      const uint64_t warps_target = (uint64_t)tb_tune("TB_MSM_SUB_WARPS_PER_SM", 16) * (uint64_t)ctx->sm_count;
+      const uint64_t warps_target = (uint64_t)MSM_SUB_WARPS_PER_SM * (uint64_t)ctx->sm_count;
       while (lpb_log < 5 && ((nb_total64 << (lpb_log + 1)) >> 5) <= warps_target && (1ull << lpb_log) < avg_units) ++lpb_log; }
     const uint32_t sub_units = 4u << lpb_log;
     uint64_t max_mid = (max_entries >> chunk_log) / sub_units + 1;   // buckets with more than sub_units * chunk entries
@@ -380,11 +381,8 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
     DevBuf<Xyzz<B>> partial(ctx, max_units);
     ctx->work[PC_MSM_ACCUM] += 10.5 * (double)max_entries * 0.97;                 // XYZZ mixed additions (upper bound: every digit non-zero)
     ps.reset(); ps.reset(new ProfScope(ctx, PC_MSM_ACCUM));
-    { const unsigned ag = (unsigned)((max_units + 127) / 128);
-      const int minb = tb_tune("TB_MSM_ACCUM_MINB", 4);
-      if (minb >= 6) msm_accum_kernel<B, 6><<<ag, 128, 0, st>>>(bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total, 1u << chunk_log, entries.get(), partial.get());
-      else if (minb == 5) msm_accum_kernel<B, 5><<<ag, 128, 0, st>>>(bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total, 1u << chunk_log, entries.get(), partial.get());
-      else msm_accum_kernel<B, 4><<<ag, 128, 0, st>>>(bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total, 1u << chunk_log, entries.get(), partial.get()); }
+    msm_accum_kernel<B><<<(unsigned)((max_units + 127) / 128), 128, 0, st>>>(bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total,
+                                                                            1u << chunk_log, entries.get(), partial.get());
     TB_LAUNCH_CHECK();
     ps.reset(); ps.reset(new ProfScope(ctx, PC_MSM_REDUCE));
     msm_combine_sub_kernel<B><<<(unsigned)((((uint64_t)nb_total << lpb_log) + 127) / 128), 128, 0, st>>>(unit_off.get(), partial.get(), nb_total, lpb_log,
@@ -398,8 +396,7 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
   }
   ps.reset(new ProfScope(ctx, PC_MSM_REDUCE));
 
-  const int seg_t = tb_tune("TB_MSM_SEG", MSM_SEG);
-  const int seg = NB < seg_t ? NB : seg_t;
+  const int seg = NB < MSM_SEG ? NB : MSM_SEG;
   const int nt = NB / seg;
   const uint32_t groups = (uint32_t)K * wsep;
   Aff<B>* const aff_out = reinterpret_cast<Aff<B>*>(cfg_in.affine_out);
@@ -471,30 +468,5 @@ template <class B> void points_to_affine(Ctx* ctx, const Xyzz<B>* acc, int K, Af
 }
 template void points_to_affine<Fq>(Ctx*, const Xyzz<Fq>*, int, Aff<Fq>*);
 template void points_to_affine<Fp>(Ctx*, const Xyzz<Fp>*, int, Aff<Fp>*);
-
-// ---------------------------------------------------------------- finalisation: + sum extra_scalar * extra_base, to affine
-template <class B, class S>
-__global__ void points_finalize_kernel(const Xyzz<B>* __restrict__ acc, int K, const S* __restrict__ extra_scalars,
-                                       const Aff<B>* __restrict__ extra_bases, int n_extra, Aff<B>* __restrict__ out) {
-  int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= K) return;
-  Xyzz<B> p = acc[k];
-  for (int j = 0; j < n_extra; ++j) {
-    S s = extra_scalars[(size_t)k * n_extra + j].from_mont();
-    if (s.is_zero()) continue;
-    Xyzz<B> t = scalar_mul(extra_bases[j], s.l);
-    p.add(t);
-  }
-  out[k] = p.to_affine();
-}
-
-template <class B, class S>
-void points_finalize(Ctx* ctx, const Xyzz<B>* acc, int K, const S* extra_scalars, const Aff<B>* extra_bases, int n_extra, Aff<B>* out) {
-  points_finalize_kernel<B, S><<<(K + 31) / 32, 32, 0, ctx->stream>>>(acc, K, extra_scalars, extra_bases, n_extra, out);
-  TB_LAUNCH_CHECK();
-  ctx->launches++;
-}
-template void points_finalize<Fq, Fp>(Ctx*, const Xyzz<Fq>*, int, const Fp*, const Aff<Fq>*, int, Aff<Fq>*);
-template void points_finalize<Fp, Fq>(Ctx*, const Xyzz<Fp>*, int, const Fq*, const Aff<Fp>*, int, Aff<Fp>*);
 
 }  // namespace tb

@@ -37,6 +37,7 @@
 namespace tb {
 
 constexpr int BA_THREADS = 256;
+constexpr int BA_M = 32;                        // pairs per thread of a round (16 is faster on sparse witness columns, slower on dense scalars: DESIGN §8)
 constexpr int BA_BWD_MINB = 3;                  // resident CTAs per SM of the backward kernel
 constexpr int BA_MAX_NB = 4096;
 constexpr int SORT_THREADS = 1024;
@@ -249,17 +250,17 @@ __global__ void __launch_bounds__(BA_THREADS) msm_ba_count_kernel(const uint32_t
 }
 
 // ---- 2a. forward: classify every pair, prefix products of the denominators (to global memory), product tree of the CTA (to
-// global memory).  A CTA owns M * BA_THREADS consecutive output items of one MSM; thread t owns items Q0 + i * BA_THREADS + t.
+// global memory).  A CTA owns BA_M * BA_THREADS consecutive output items of one MSM; thread t owns items Q0 + i * BA_THREADS + t.
 // Per item q it stores meta[q] = in0 | kind << META_KIND_SHIFT, and in round 0 the two signed table indices of the pair (eidx),
 // so that the backward kernel neither searches nor classifies again and gathers the table points without the entries load.
-template <class B, bool FIRST, int M>
+template <class B, bool FIRST>
 __global__ void __launch_bounds__(BA_THREADS) msm_ba_fwd_kernel(const uint32_t* __restrict__ counts0, int NB, int round, const uint32_t* __restrict__ entries,
                                                                  const Aff<B>* __restrict__ table, const B* __restrict__ items_in, long long cap_in, long long cap_out,
                                                                  B* __restrict__ pre, B* __restrict__ tree, uint32_t* __restrict__ meta, uint2* __restrict__ eidx,
                                                                  const uint32_t* __restrict__ n_items, int R) {
   extern __shared__ __align__(16) uint8_t ba_smem[];
   const int k = blockIdx.y, t = threadIdx.x;
-  const uint32_t Q0 = blockIdx.x * (M * BA_THREADS);
+  const uint32_t Q0 = blockIdx.x * (BA_M * BA_THREADS);
   if (Q0 >= n_items[(long long)k * (R + 1) + round + 1]) return;   // nothing of this MSM left for this CTA (uniform over the CTA)
   RoundOffsets ro; ro.build(ba_smem, counts0 + (long long)k * NB, NB, round);
   const uint32_t* ent_k = entries + (long long)k * cap_in;
@@ -270,7 +271,7 @@ __global__ void __launch_bounds__(BA_THREADS) msm_ba_fwd_kernel(const uint32_t* 
   B acc = B::one();
   int hint = 0;
 #pragma unroll 1
-  for (int i = 0; i < M; ++i) {
+  for (int i = 0; i < BA_M; ++i) {
     const uint32_t q = Q0 + (uint32_t)i * BA_THREADS + t;
     if (q >= ro.n_next) break;
     uint32_t in0; bool two; ro.locate(q, NB, in0, two, hint);
@@ -313,13 +314,13 @@ __global__ void msm_ba_inv_kernel(B* __restrict__ tree, uint32_t n_trees) {
 
 // ---- 2c. backward: push the inverted root down the tree, then walk every thread's pairs back and write the sums.
 // BA_BWD_MINB resident CTAs per SM (80 registers): faster on H100 than 2 (more registers, fewer warps) or 4 (64 registers, spills).
-template <class B, bool FIRST, int M>
+template <class B, bool FIRST>
 __global__ void __launch_bounds__(BA_THREADS, BA_BWD_MINB) msm_ba_bwd_kernel(const Aff<B>* __restrict__ table, const B* __restrict__ items_in, long long cap_in,
                                                                  B* __restrict__ items_out, long long cap_out, const B* __restrict__ tree,
                                                                  const uint32_t* __restrict__ meta, const uint2* __restrict__ eidx, const uint32_t* __restrict__ n_items, int round, int R) {
   extern __shared__ __align__(16) uint8_t ba_smem[];
   const int k = blockIdx.y, t = threadIdx.x;
-  const uint32_t Q0 = blockIdx.x * (M * BA_THREADS);
+  const uint32_t Q0 = blockIdx.x * (BA_M * BA_THREADS);
   const uint32_t n_next = n_items[(long long)k * (R + 1) + round + 1];
   if (Q0 >= n_next) return;
   B* nd = reinterpret_cast<B*>(ba_smem);   // [2 * BA_THREADS]
@@ -341,7 +342,7 @@ __global__ void __launch_bounds__(BA_THREADS, BA_BWD_MINB) msm_ba_bwd_kernel(con
   // the prefix products of the forward kernel sit in the y plane of the output: slot q is read (plain, coherent load) by this
   // thread before it writes out.y[q] over it
   const B* pre_k = out.x + cap_out;
-  int last = M - 1;
+  int last = BA_M - 1;
   while (last >= 0 && Q0 + (uint32_t)last * BA_THREADS + t >= n_next) --last;
 #pragma unroll 1
   for (int i = last; i >= 0; --i) {
@@ -403,21 +404,16 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// one reduction round = forward, root inversion, backward; M (pairs per thread) is a tuning parameter: 32 is faster on dense
-// scalars, 16 on sparse witness columns (more CTAs share out the few pairs of the later rounds)
-template <class B, bool FIRST, int M>
-static void launch_round_t(Ctx* ctx, dim3 grid, size_t fwd_smem, size_t bwd_smem, const uint32_t* counts, int NB, int r, const uint32_t* entries, const Aff<B>* table, const B* in,
-                           long long cap_in, B* out, long long cap_out, B* pre, B* tree, uint32_t* meta, uint2* eidx, const uint32_t* n_items, int R, uint32_t n_trees) {
+// one reduction round = forward, root inversion, backward
+template <class B, bool FIRST>
+static void launch_round(Ctx* ctx, dim3 grid, size_t fwd_smem, size_t bwd_smem, const uint32_t* counts, int NB, int r, const uint32_t* entries, const Aff<B>* table, const B* in,
+                         long long cap_in, B* out, long long cap_out, B* pre, B* tree, uint32_t* meta, uint2* eidx, const uint32_t* n_items, int R, uint32_t n_trees) {
   cudaStream_t st = ctx->stream;
-  ctx->opt_in_smem(msm_ba_fwd_kernel<B, FIRST, M>, fwd_smem);
-  ctx->opt_in_smem(msm_ba_bwd_kernel<B, FIRST, M>, bwd_smem);
-  msm_ba_fwd_kernel<B, FIRST, M><<<grid, BA_THREADS, fwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, eidx, n_items, R);
+  ctx->opt_in_smem(msm_ba_fwd_kernel<B, FIRST>, fwd_smem);
+  ctx->opt_in_smem(msm_ba_bwd_kernel<B, FIRST>, bwd_smem);
+  msm_ba_fwd_kernel<B, FIRST><<<grid, BA_THREADS, fwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, eidx, n_items, R);
   msm_ba_inv_kernel<B><<<(n_trees + 63) / 64, 64, 0, st>>>(tree, n_trees);
-  msm_ba_bwd_kernel<B, FIRST, M><<<grid, BA_THREADS, bwd_smem, st>>>(table, in, cap_in, out, cap_out, tree, meta, eidx, n_items, r, R);
-}
-template <class B, typename... A> static void launch_round(Ctx* ctx, int M, bool first, A... a) {
-  if (M == 32) { if (first) launch_round_t<B, true, 32>(ctx, a...); else launch_round_t<B, false, 32>(ctx, a...); }
-  else { if (first) launch_round_t<B, true, 16>(ctx, a...); else launch_round_t<B, false, 16>(ctx, a...); }
+  msm_ba_bwd_kernel<B, FIRST><<<grid, BA_THREADS, bwd_smem, st>>>(table, in, cap_in, out, cap_out, tree, meta, eidx, n_items, r, R);
 }
 
 bool msm_batch_applicable(int N, int K, const MsmConfig& cfg, int c) {
@@ -457,8 +453,7 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
   ctx->opt_in_smem(msm_sort_kernel<S, 13>, sort_smem);
   ctx->opt_in_smem(msm_sort_kernel<S, 0>, sort_smem);
   ctx->opt_in_smem(msm_ba_finish_kernel<B>, fin_smem);
-  const int Mv = tb_tune("TB_MSM_BA_M", 32) >= 32 ? 32 : 16;
-  const long long pairs_per_cta = (long long)Mv * BA_THREADS;
+  const long long pairs_per_cta = (long long)BA_M * BA_THREADS;
   const unsigned ctas1 = (unsigned)((cap[1] + pairs_per_cta - 1) / pairs_per_cta);
   DevBuf<B> tree(ctx, (size_t)Kc * ctas1 * 2 * BA_THREADS);
   DevBuf<uint32_t> meta(ctx, (size_t)Kc * cap[1]), n_items(ctx, (size_t)Kc * (R + 1));
@@ -485,8 +480,8 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
         const unsigned gx = (unsigned)((cap[r + 1] + pairs_per_cta - 1) / pairs_per_cta);
         dim3 grid(gx, kc);
         const uint32_t n_trees = gx * (uint32_t)kc;
-        launch_round<B>(ctx, Mv, r == 0, grid, fwd_smem, bwd_smem, counts.get(), NB, r, entries.get(), table, in, r == 0 ? cap0 : cap[r], out, cap[r + 1], out + cap[r + 1], tree.get(),
-                        meta.get(), eidx, n_items.get(), R, n_trees);
+        (r == 0 ? launch_round<B, true> : launch_round<B, false>)(ctx, grid, fwd_smem, bwd_smem, counts.get(), NB, r, entries.get(), table, in, r == 0 ? cap0 : cap[r], out,
+                                                                  cap[r + 1], out + cap[r + 1], tree.get(), meta.get(), eidx, n_items.get(), R, n_trees);
         TB_LAUNCH_CHECK(); ctx->launches += 3;
       }
       const B* last = (R & 1) ? itA.get() : itB.get();

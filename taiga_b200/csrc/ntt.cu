@@ -117,8 +117,8 @@ __global__ void __launch_bounds__(NTT_THREADS) ntt_pass_kernel(const F* __restri
   }
 }
 
-static void ntt_plan(int logn, int* rs, int* npass, int tile_log) {
-  if (logn <= tile_log) { rs[0] = logn; *npass = 1; return; }
+static void ntt_plan(int logn, int* rs, int* npass) {
+  if (logn <= NTT_TILE_LOG) { rs[0] = logn; *npass = 1; return; }
   int np = logn > 16 ? (logn + 8) / 9 : 2;
   int base = logn / np, rem = logn % np;
   for (int i = 0; i < np; ++i) rs[i] = base + (i < rem ? 1 : 0);
@@ -139,8 +139,7 @@ void ntt_run(Ctx* ctx, int logn, bool inverse, const F* in, F* out, F* scratch, 
   NttArgs<F> a;
   a.tw = inverse ? field_tables<F>(ctx).inv : field_tables<F>(ctx).fwd;
   a.logn = logn;
-  const int tile_log = tb_tune("TB_NTT_TILE_LOG", NTT_TILE_LOG);
-  ntt_plan(logn, a.rs, &a.npass, tile_log);
+  ntt_plan(logn, a.rs, &a.npass);
   NttHook<F> none; none.use_zeta = 0; none.k = 0; none.use_const = 0; none.mod_bits = TW_LOG;
   a.pre = pre ? *pre : none;
   a.post = post ? *post : none;
@@ -153,7 +152,7 @@ void ntt_run(Ctx* ctx, int logn, bool inverse, const F* in, F* out, F* scratch, 
   for (int p = 0; p < a.npass; ++p) {
     a.pass = p; a.r = a.rs[p]; sh -= a.r; a.sh = sh; a.last = (p == a.npass - 1);
     int lanes_log = logn - a.r;
-    a.logT = tile_log - a.r < lanes_log ? tile_log - a.r : lanes_log;
+    a.logT = NTT_TILE_LOG - a.r < lanes_log ? NTT_TILE_LOG - a.r : lanes_log;
     if (a.logT < 0) a.logT = 0;
     const F* src = (p == 0) ? in : scratch;
     F* dst = a.last ? out : scratch;

@@ -27,7 +27,7 @@ static Fp* dev_alloc_fp(size_t count) { Fp* p = nullptr; TB_CUDA(cudaMalloc(&p, 
 
 static NttHook<Fp> coset_hook(const Circuit& C, int k1, bool inverse) {
   NttHook<Fp> h; h.use_const = 0; h.mod_bits = C.ext_k; h.k = (uint32_t)k1;
-  if (!inverse) { h.use_zeta = 1; h.z1 = C.zeta; h.z2 = C.zeta.sqr(); if (C.coset_pre) h.table = C.coset_pre + (size_t)k1 * C.n; }
+  if (!inverse) { h.use_zeta = 1; h.z1 = C.zeta; h.z2 = C.zeta.sqr(); h.table = C.coset_pre + (size_t)k1 * C.n; }
   else { h.use_zeta = 0; h.z1 = Fp::one(); h.z2 = Fp::one(); }
   return h;
 }
@@ -111,15 +111,13 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   { std::vector<Fp> cm(C.nconsts);
     for (uint32_t i = 0; i < C.nconsts; ++i) { Fp v; memcpy(v.l, C.consts_bytes.data() + 32 * i, 32); cm[i] = v.to_mont(); }
     C.consts = dev_upload(cm); }
-  auto q2 = [](const std::vector<tb_query>& qs) { std::vector<int2> v; for (auto& q : qs) v.push_back(make_int2((int)q.column, q.rotation)); return v; };
-  C.d_aq = dev_upload(q2(C.aq)); C.d_fq = dev_upload(q2(C.fq)); C.d_iq = dev_upload(q2(C.iq));
   { std::vector<int2> pc; for (auto& c : C.perm) pc.push_back(make_int2((int)c.kind, (int)c.index)); C.d_perm = dev_upload(pc); }
 
-  { // per-element factors of the forward coset hooks (one multiplication per coefficient instead of up to two and a table walk)
-    Fp* tab = dev_alloc_fp((size_t)C.R * n);
-    for (int k1 = 0; k1 < C.R; ++k1) { NttHook<Fp> h = coset_hook(C, k1, false); ntt_hook_table<Fp>(ctx, h, false, tab + (size_t)k1 * n, (int)n); }
+  { // per-element factors of the forward coset hooks (one multiplication per coefficient instead of up to two and a table walk);
+    // ntt_hook_table computes them from the hook without its table
+    C.coset_pre = dev_alloc_fp((size_t)C.R * n);
+    for (int k1 = 0; k1 < C.R; ++k1) { NttHook<Fp> h = coset_hook(C, k1, false); ntt_hook_table<Fp>(ctx, h, false, C.coset_pre + (size_t)k1 * n, (int)n); }
     ctx->sync();
-    if (tb_tune("TB_NTT_HOOK_TABLE", 1)) C.coset_pre = tab; else cudaFree(tab);
   }
   DevBuf<Fp> scratch(ctx, std::max<size_t>(3, std::max<size_t>(C.nf, C.P)) * n);
   auto load_cols = [&](const uint8_t* src, size_t cnt, Fp*& vals, Fp*& polys, Fp*& cosets) {
@@ -164,13 +162,14 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
                                       lo.size(), C.R / 2, t_lo[0].ninstr, t_all[0].ninstr, C.split ? "on" : "off");
       for (auto& qp : t_all) if (qp.dev) cudaFree(qp.dev);
       for (auto& qp : t_lo) if (qp.dev) cudaFree(qp.dev); }
-    for (int parts : {1, 2, 4, 8, 16}) {
-      q_compile_gates_split(&d, C.split ? hi : all, parts, &C.gate_parts[parts]);
-      if (C.split) q_compile_gates_split(&d, lo, parts, &C.gate_parts_lo[parts]);
+    for (int big = 0; big < 2; ++big) {
+      q_compile_gates_split(&d, C.split ? hi : all, Circuit::gate_nparts[big], &C.gate_parts[big]);
+      if (C.split) q_compile_gates_split(&d, lo, Circuit::gate_nparts[big], &C.gate_parts_lo[big]);
     }
     if (getenv("TB_DEBUG")) {
-      for (auto* m : {&C.gate_parts, &C.gate_parts_lo})
-        for (auto& kv : *m) { fprintf(stderr, "[tb]   %s %d parts:", m == &C.gate_parts ? "all/high" : "low", kv.first); for (auto& qp : kv.second) fprintf(stderr, " %d/%d", qp.ninstr, qp.nregs); fprintf(stderr, "\n"); }
+      for (auto* m : {C.gate_parts, C.gate_parts_lo})
+        for (int big = 0; big < 2; ++big) if (!m[big].empty()) {
+          fprintf(stderr, "[tb]   %s %d parts:", m == C.gate_parts ? "all/high" : "low", Circuit::gate_nparts[big]); for (auto& qp : m[big]) fprintf(stderr, " %d/%d", qp.ninstr, qp.nregs); fprintf(stderr, "\n"); }
     }
     q_compile_lookups(&d, &C.prog_lookups); }
 
@@ -316,8 +315,9 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   WsAlloc ws{ctx, C, pws.blocks};
   std::vector<void*>& tables = pws.tables;
   size_t table_cur = 0;
-  // uploads a small host table once per (circuit, context, B); later calls reuse the device copy.  The contents are compared with
-  // what was uploaded (they change only when a TB_* tuning knob changes between calls) and refreshed in stream order if they differ.
+  // uploads a small host table once per (circuit, context, B); later calls reuse the device copy.  The contents follow from the
+  // circuit and B alone; they are still compared with what was uploaded (a cheap guard should a table come to depend on anything
+  // else) and refreshed in stream order if they differ.
   auto cached_upload = [&](const void* host, size_t bytes) -> void* {
     const uint8_t* hb = static_cast<const uint8_t*>(host);
     if (table_cur == tables.size()) {
@@ -500,17 +500,14 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   // Constraint-parallel split of the gate program.  More parts = shorter per-thread chains (latency at small batches) AND
   // fewer live temporaries per part = smaller shared-memory register file = higher occupancy (ncu: 6 warps/SM with one
   // 26-register program vs 20 warps/SM with eight <=11-register parts), for ~15% more instructions in total.
-  int gparts = tb_tune("TB_Q_PARTS", B >= 8 ? 4 : 8);   // small batches: more, shorter programs (latency); large ones: less duplicated work
-  if (gparts != 1 && gparts != 2 && gparts != 4 && gparts != 8 && gparts != 16) gparts = 8;
-  const std::vector<QProgram>& gprogs = C.gate_parts.at(gparts);
-  const std::vector<QProgram>* lprogs = C.split ? &C.gate_parts_lo.at(gparts) : nullptr;
+  const std::vector<QProgram>& gprogs = C.gate_parts[B >= 8];
+  const std::vector<QProgram>* lprogs = C.split ? &C.gate_parts_lo[B >= 8] : nullptr;
   { Prog p; p.op(S_CONST, V_YTAB, 0, 0, 0); p.op(S_COPY, V_YTAB + 1, V_Y);
     for (int i = 2; i < YTAB; ++i) p.op(S_MUL, V_YTAB + i, V_YTAB + i - 1, V_Y);
     run_prog(p); }
   const int J = (int)C.num_constraints;
   WBuf<Fp> hext = ws.buf<Fp>((size_t)B * R * n), hcoef = ws.buf<Fp>((size_t)B * C.pieces * n);
   { WBuf<Fp> c_lkA = ws.buf<Fp>((size_t)B * L1 * n), c_lkS = ws.buf<Fp>((size_t)B * L1 * n), gate = ws.buf<Fp>((size_t)Q_MAX_PARTS * B * n), V = ws.buf<Fp>((size_t)B * R * n);
-    Fp* const c_adv0 = cosets.get() + (size_t)O_ADV * n;
     const int Rlo = C.split ? R / 2 : 0;
     // ---- low-degree constraints: every second sub-coset only.  Their sum H_lo is interpolated (Rlo * n coefficients) and divided by
     // X^n - 1 in coefficient form, H_lo = q_lo (X^n - 1) + r_lo; q_lo goes straight into h, r_lo (n coefficients) joins the numerator
@@ -549,7 +546,6 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       if (C.split) ntt_run<Fp>(ctx, k, false, rlo_poly.get(), rlo_coset.get(), scratch.get(), B, nn, nn, &h, nullptr);
       Fp* const c_adv = ck + (size_t)O_ADV * n; Fp* const c_inst = ck + (size_t)O_INST * n; Fp* const c_pz = ck + (size_t)O_PZ * n;
       Fp* const c_lz = ck + (size_t)O_LZ * n; Fp* const c_lpin = ck + (size_t)O_LPIN * n; Fp* const c_lptab = ck + (size_t)O_LPTAB * n;
-      (void)c_adv0;
       qd.adv = c_adv; qd.adv_pstride = PS; qd.inst = c_inst; qd.inst_pstride = PS;
       qd.fix = C.fixed_cosets; qd.R = R; qd.k1 = k1; qd.lkA = c_lkA.get(); qd.lkS = c_lkS.get();
       qd.gate_out = gate.get(); qd.gate_pstride = nn;

@@ -27,7 +27,7 @@ struct QProgram {           // compiled once per circuit (host), resident on the
 // The (sorted) constraint subset `subset` split into `parts` groups of similar cost, one program each (row-parallel AND
 // constraint-parallel evaluation).  Folds are gap-aware: program p yields S_p = sum_{j in p} y^(last_p - j) e_j, so any
 // set of programs combines as sum_p y^(J - 1 - last_p) S_p, whatever subset of the J constraints each one holds.
-constexpr int Q_MAX_PARTS = 16;
+constexpr int Q_MAX_PARTS = 8;
 void q_compile_gates_split(const tb_cs_desc* cs, const std::vector<uint32_t>& subset, int parts, std::vector<QProgram>* out);
 // polynomial degree of every constraint (a column query counts 1): decides which sub-cosets a constraint must be evaluated on
 std::vector<int> q_constraint_degrees(const tb_cs_desc* cs);

@@ -230,7 +230,9 @@ void q_compile_lookups(const tb_cs_desc* cs, QProgram* out) {
 // [nregs + 2][T] x 32 B (slot nregs = the y / theta fold accumulator, slot nregs + 1 = the group / table fold): the loop carries
 // no 256-bit value in registers, which kept the compiler from shuffling 16-24 registers on every interpreted instruction
 // (ncu source view of the previous version: 30 % of the executed instructions were MOV / CS2R / SEL / BRA).
-__global__ void __launch_bounds__(128) q_interp_kernel(QPartList pl, int nregs, QData d) {
+// `pl` is indexed by blockIdx.z: __grid_constant__ keeps those loads in the parameter bank, where ptxas would otherwise copy the
+// part list to the stack of every thread.
+__global__ void __launch_bounds__(128) q_interp_kernel(const __grid_constant__ QPartList pl, int nregs, QData d) {
   const uint4* __restrict__ prog = reinterpret_cast<const uint4*>(pl.prog[blockIdx.z]);
   const int ninstr = pl.ninstr[blockIdx.z];
   extern __shared__ uint4 q_smem[];
@@ -300,8 +302,7 @@ static void q_launch(Ctx* c, const QPartList& pl, int nregs, const QData& d, int
   c->opt_in_smem(q_interp_kernel, 96 * 1024);
   // T threads evaluate T rows; the register file [nregs + 2][T] x 32 B lives in shared memory
   int T = (96 * 1024) / ((nregs + 2) * 32);
-  const int tmax = tb_tune("TB_Q_THREADS", 128);
-  T = T >= tmax ? tmax : (T / 16) * 16;
+  T = T >= 128 ? 128 : (T / 16) * 16;
   TB_REQUIRE(T >= 16 && T <= 128, "constraint program register file does not fit shared memory");
   while (T > d.n && T > 1) T >>= 1;
   const size_t smem = (size_t)(nregs + 2) * T * 32;

@@ -2,7 +2,6 @@
 // Replaces halo2_proofs `poly::commitment::Params<vesta::Affine>` (EXT) as loaded by SETUP_PARAMS_MAP
 // (taiga_halo2/src/constant.rs:128-139) and its `commit` / `commit_lagrange` methods (SURVEY.md §8a H1, App. E.4).
 #pragma once
-#include <cstdlib>
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -22,8 +21,8 @@ struct Srs {
   static Srs* load(Ctx* ctx, uint32_t k, const uint8_t* g, const uint8_t* gl, const uint8_t* w, const uint8_t* u) {
     Srs* s = new Srs();
     s->ctx = ctx; s->k = k; s->n = size_t(1) << k;
-    int c = (int)k - 2; if (c < 4) c = 4; if (c > 13) c = 13;  // 13: 4096 buckets per MSM at k = 15 (see msm.cu MSM_FIXED_C)
-    if (const char* e = getenv("TB_FIXED_C")) { int v = atoi(e); if (v >= 4 && v <= 15) c = v; }  // tuning knob for experiments
+    // 13 at k = 15: 4096 buckets per MSM, 20 table windows (measured best of 11/12/13/16 at k = 15)
+    int c = (int)k - 2; if (c < 4) c = 4; if (c > 13) c = 13;
     s->c = c; s->W = (256 + c - 1) / c;
     size_t n = s->n;
     try {

@@ -216,7 +216,6 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     { Fp repr = C.vk_repr.to_mont(); tr.common_scalar(repr); }
     bool ok = true;
     const uint8_t* ib = instance + 32 * inst_total * p;
-    std::vector<Fp> inst_vals_chk;  // canonical check of the public inputs
     for (size_t i = 0; i < inst_total && ok; ++i) { Fp t; ok = canonical<Fp>(ib + 32 * i, t); }
     if (!ok) continue;
     // commitment table for this proof: id -> point

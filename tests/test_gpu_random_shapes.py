@@ -14,9 +14,7 @@ from test_random_shapes_oracle import SHAPES, shape
 pytestmark = pytest.mark.gpu
 
 # the knob sets of test_tuning_knobs_do_not_change_results, plus the quotient without the degree split
-KNOB_SETS = [{"TB_MSM_BA_MIN_TERMS": "0"}, {"TB_MSM_BA_MIN_TERMS": "0", "TB_MSM_BA_ROUNDS": "2", "TB_MSM_BA_CHUNK": "3"},
-             {"TB_Q_PARTS": "1", "TB_Q_THREADS": "32"}, {"TB_Q_PARTS": "16", "TB_MSM_UNITS_PER_SM": "1", "TB_MSM_SUB_WARPS_PER_SM": "1"},
-             {"TB_NTT_TILE_LOG": "8", "TB_MSM_ACCUM_MINB": "6", "TB_MSM_SEG": "2"}, {"TB_Q_SPLIT": "0"}]
+KNOB_SETS = [{"TB_MSM_BA_MIN_TERMS": "0"}, {"TB_MSM_BA_MIN_TERMS": "0", "TB_MSM_BA_ROUNDS": "2", "TB_MSM_BA_CHUNK": "3"}, {"TB_Q_SPLIT": "0"}]
 SPLIT_SHAPE = ("boundary", "split_mixed_degrees")
 
 

@@ -176,7 +176,7 @@ def main():
     from taiga_b200 import lib
     os.environ["TB_MSM_BA_MIN_TERMS"] = "0"
     R = int(os.environ.get("TB_MSM_BA_ROUNDS", 10))
-    M = 32 if int(os.environ.get("TB_MSM_BA_M", 32)) >= 32 else 16   # as msm_batch_buckets rounds the knob
+    M = 32   # pairs per thread (msm_batch.cu BA_M)
     raw = np.fromfile(os.path.join(ROOT, "tests", "golden", "srs_k15_affine.bin"), dtype=np.uint8).reshape(-1, 64)
     ctx = lib.Context(0)
     srs = ctx.load_srs(15, raw[:N15], raw[N15:2 * N15], raw[2 * N15], raw[2 * N15 + 1])

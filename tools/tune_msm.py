@@ -15,7 +15,7 @@ bl = np.zeros((K, 32), np.uint8)
 os.environ["TB_MSM_BA_MIN_TERMS"] = "0"
 ref = None
 CONFIGS = None
-for cfg in CONFIGS or [{}, {"TB_MSM_BA_M": "16"}, {"TB_MSM_BA_ROUNDS": "8"}, {"TB_MSM_BA_ROUNDS": "9"}, {"TB_MSM_BA_CHUNK": "704"}, {}]:
+for cfg in CONFIGS or [{}, {"TB_MSM_BA_ROUNDS": "8"}, {"TB_MSM_BA_ROUNDS": "9"}, {"TB_MSM_BA_CHUNK": "704"}, {}]:
     os.environ.update(cfg)
     out = srs.commit(s, bl, lagrange=True, batch=K)
     ctx.prof_enable(True)
