@@ -6,7 +6,8 @@
 #include <cstdio>
 #include <stdexcept>
 #include <string>
-#include <set>
+#include <map>
+#include <mutex>
 #include <vector>
 #include "curve.cuh"
 
@@ -49,6 +50,18 @@ struct ProfRec { int cat; cudaEvent_t a, b; };
 // quotient's degree split at circuit load.  Every other launch choice is a constant of the code.
 inline int tb_tune(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 
+// Opt a kernel into more than 48 KB of dynamic shared memory on the current device.  The attribute belongs to the (function,
+// device) pair, which every context of the device shares, and a kernel may need more on a later call (msm_sort_kernel's
+// histogram grows with the window), so the attribute only ever grows, to the largest size a launch on the device asked for.
+// The table is never destroyed: a thread of the host program may still launch while the process exits.
+inline void opt_in_smem_device(int device, const void* kernel, size_t bytes) {
+  static std::mutex* mu = new std::mutex;
+  static auto* opted = new std::map<std::pair<int, const void*>, size_t>;
+  std::lock_guard<std::mutex> lock(*mu);
+  size_t& have = (*opted)[{device, kernel}];
+  if (bytes > have) { TB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)); have = bytes; }
+}
+
 struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -75,13 +88,7 @@ struct Ctx {
     return reinterpret_cast<T*>(p);
   }
   void free(void* p) { if (p) cudaFreeAsync(p, stream); }
-  // Opt a kernel into more than 48 KB of dynamic shared memory.  The attribute belongs to the (function, device) pair, so the
-  // "already done" set lives in the context (= one device), not in a process-wide static.
-  std::set<const void*> smem_opted;
-  template <class K> void opt_in_smem(K kernel, size_t bytes) {
-    if (smem_opted.insert(reinterpret_cast<const void*>(kernel)).second)
-      TB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  }
+  template <class K> void opt_in_smem(K kernel, size_t bytes) { opt_in_smem_device(device, reinterpret_cast<const void*>(kernel), bytes); }
   void sync() { TB_CUDA(cudaStreamSynchronize(stream)); }
 };
 
