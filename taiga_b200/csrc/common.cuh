@@ -7,6 +7,7 @@
 #include <stdexcept>
 #include <string>
 #include <map>
+#include <utility>
 #include <mutex>
 #include <vector>
 #include "curve.cuh"
@@ -23,7 +24,6 @@ struct ConstraintError : std::runtime_error { using std::runtime_error::runtime_
     if (_e != cudaSuccess)                                                                              \
       throw tb::CudaError(std::string(#expr) + " failed: " + cudaGetErrorString(_e) + " at " + __FILE__ + ":" + std::to_string(__LINE__)); \
   } while (0)
-#define TB_LAUNCH_CHECK() TB_CUDA(cudaGetLastError())
 #define TB_REQUIRE(cond, msg) do { if (!(cond)) throw std::invalid_argument(std::string(msg) + " (" #cond ")"); } while (0)
 
 // NTT twiddle tables: powers of the 2^24-th root of unity, two-level (SURVEY E.3; tables are 2 x 128 KiB per
@@ -91,6 +91,25 @@ struct Ctx {
   template <class K> void opt_in_smem(K kernel, size_t bytes) { opt_in_smem_device(device, reinterpret_cast<const void*>(kernel), bytes); }
   void sync() { TB_CUDA(cudaStreamSynchronize(stream)); }
 };
+
+// Every kernel of the library is launched here: on the context's stream, as clusters of `cluster` CTAs along x when
+// cluster > 1, checked at once (so a failure names the kernel that failed) and counted in `launches`.
+template <class... P, class... A>
+void launch_cluster(Ctx* c, unsigned cluster, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  cudaLaunchAttribute at = {};
+  at.id = cudaLaunchAttributeClusterDimension; at.val.clusterDim.x = cluster; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+  const cudaLaunchConfig_t cfg = {grid, block, smem, c->stream, &at, cluster > 1 ? 1u : 0u};
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+  if (e == cudaSuccess) e = cudaGetLastError();   // or an error an earlier call left pending
+  if (e != cudaSuccess) {
+    const char* name = "?"; cudaFuncGetName(&name, kernel);
+    throw CudaError(std::string("launch of ") + name + " failed: " + cudaGetErrorString(e));
+  }
+  c->launches++;
+}
+template <class... P, class... A> void launch(Ctx* c, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  launch_cluster(c, 1, kernel, grid, block, smem, std::forward<A>(args)...);
+}
 
 // records a pair of CUDA events on the context's stream around a group of launches (only when profiling is on)
 struct ProfScope {

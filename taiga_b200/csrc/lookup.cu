@@ -70,15 +70,12 @@ void sort_keys(Ctx* c, Fp* keys, int n, int arrays) {
   c->opt_in_smem(bitonic_local_kernel, BS_TILE * 32);
   int tile = n < BS_TILE ? n : BS_TILE;
   dim3 lg(n / tile, arrays);
-  bitonic_local_kernel<<<lg, BS_THREADS, tile * 32, c->stream>>>(keys, n, tile, 1, 0, 0);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, bitonic_local_kernel, lg, BS_THREADS, tile * 32, keys, n, tile, 1, 0, 0);
   for (int k = tile << 1; k <= n; k <<= 1) {
     for (int j = k >> 1; j >= tile; j >>= 1) {
-      bitonic_global_kernel<<<dim3((n / 2 + 255) / 256, arrays), 256, 0, c->stream>>>(keys, n, k, j);
-      TB_LAUNCH_CHECK(); c->launches++;
+      launch(c, bitonic_global_kernel, dim3((n / 2 + 255) / 256, arrays), 256, 0, keys, n, k, j);
     }
-    bitonic_local_kernel<<<lg, BS_THREADS, tile * 32, c->stream>>>(keys, n, tile, 0, k, tile >> 1);
-    TB_LAUNCH_CHECK(); c->launches++;
+    launch(c, bitonic_local_kernel, lg, BS_THREADS, tile * 32, keys, n, tile, 0, k, tile >> 1);
   }
 }
 
@@ -159,13 +156,11 @@ __global__ void __launch_bounds__(LP_THREADS) lookup_arrange_kernel(const Fp* __
 }
 
 void lookup_arrange(Ctx* c, const Fp* sortedA, const Fp* sortedT, Fp* scratch, Fp* S, int n, int usable, int arrays, uint32_t* d_err) {
-  lookup_arrange_kernel<<<arrays, LP_THREADS, 0, c->stream>>>(sortedA, sortedT, scratch, S, n, usable, d_err);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, lookup_arrange_kernel, arrays, LP_THREADS, 0, sortedA, sortedT, scratch, S, n, usable, d_err);
 }
 
 void lookup_keys(Ctx* c, Fp* keys, const Fp* vals, int n, int usable, int arrays) {
-  lookup_keys_kernel<<<dim3((n + 255) / 256, arrays), 256, 0, c->stream>>>(keys, vals, n, usable);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, lookup_keys_kernel, dim3((n + 255) / 256, arrays), 256, 0, keys, vals, n, usable);
 }
 
 }  // namespace tb

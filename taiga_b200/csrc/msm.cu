@@ -344,19 +344,16 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
   if (msm_batch_applicable(N, K, cfg_in, c)) {
     // throughput path: shared-memory counting sort per MSM + batch-affine pairwise reduction (msm_batch.cu)
     msm_batch_buckets<B, S>(ctx, scalars, scalar_bstride, bases, N, K, c, W, table_stride, reinterpret_cast<const S*>(cfg_in.extra_scalars), n_extra, buckets.get());
-    ctx->launches -= 6;   // the fixed count added below covers the latency path's sort / accumulate launches
   } else {
     DevBuf<uint32_t> counts(ctx, nb_total), offs(ctx, nb_total + 1), cursor(ctx, nb_total), entries(ctx, max_entries);
     ps.reset(new ProfScope(ctx, PC_MSM_SORT));
     counts.zero();
     dim3 dg((N + n_extra + 255) / 256, K);
     const S* extras = reinterpret_cast<const S*>(cfg_in.extra_scalars);
-    msm_digits_kernel<S, 0><<<dg, 256, 0, st>>>(scalars, scalar_bstride, N, c, W, NB, wsep, table_mode, table_stride, extras, n_extra, counts.get(), nullptr);
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_digits_kernel<S, 0>, dg, 256, 0, scalars, scalar_bstride, N, c, W, NB, wsep, table_mode, table_stride, extras, n_extra, counts.get(), nullptr);
     exclusive_scan_u32(ctx, counts.get(), offs.get(), nb_total);
     TB_CUDA(cudaMemcpyAsync(cursor.get(), offs.get(), nb_total * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-    msm_digits_kernel<S, 1><<<dg, 256, 0, st>>>(scalars, scalar_bstride, N, c, W, NB, wsep, table_mode, table_stride, extras, n_extra, cursor.get(), entries.get());
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_digits_kernel<S, 1>, dg, 256, 0, scalars, scalar_bstride, N, c, W, NB, wsep, table_mode, table_stride, extras, n_extra, cursor.get(), entries.get());
 
     // adaptive chunk: aim at ~4 waves of 512 threads per SM so that small batches still fill the machine
     uint32_t chunk_log = 3;
@@ -375,23 +372,20 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
     if (max_mid > nb_total64) max_mid = nb_total64;
     DevBuf<uint32_t> unit_count(ctx, nb_total), unit_off(ctx, nb_total + 1), mid(ctx, max_mid), heavy(ctx, max_heavy), n_lists(ctx, 2);
     n_lists.zero();
-    msm_units_kernel<<<(nb_total + 255) / 256, 256, 0, st>>>(offs.get(), nb_total, chunk_log, sub_units, unit_count.get(), mid.get(), heavy.get(), n_lists.get());
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_units_kernel, (nb_total + 255) / 256, 256, 0, offs.get(), nb_total, chunk_log, sub_units, unit_count.get(), mid.get(), heavy.get(), n_lists.get());
     exclusive_scan_u32(ctx, unit_count.get(), unit_off.get(), nb_total);
     DevBuf<Xyzz<B>> partial(ctx, max_units);
     ctx->work[PC_MSM_ACCUM] += 10.5 * (double)max_entries * 0.97;                 // XYZZ mixed additions (upper bound: every digit non-zero)
     ps.reset(); ps.reset(new ProfScope(ctx, PC_MSM_ACCUM));
-    msm_accum_kernel<B><<<(unsigned)((max_units + 127) / 128), 128, 0, st>>>(bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total,
-                                                                            1u << chunk_log, entries.get(), partial.get());
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_accum_kernel<B>, (unsigned)((max_units + 127) / 128), 128, 0, bases, base_bstride, (uint32_t)wsep * NB, offs.get(), unit_off.get(), nb_total,
+           1u << chunk_log, entries.get(), partial.get());
     ps.reset(); ps.reset(new ProfScope(ctx, PC_MSM_REDUCE));
-    msm_combine_sub_kernel<B><<<(unsigned)((((uint64_t)nb_total << lpb_log) + 127) / 128), 128, 0, st>>>(unit_off.get(), partial.get(), nb_total, lpb_log,
-                                                                                                        buckets.get());
+    launch(ctx, msm_combine_sub_kernel<B>, (unsigned)((((uint64_t)nb_total << lpb_log) + 127) / 128), 128, 0, unit_off.get(), partial.get(), nb_total, lpb_log,
+           buckets.get());
     { uint64_t g = (max_mid + 7) / 8, cap = 4ull * (uint64_t)ctx->sm_count;   // e.g. a witness column that is mostly small values
-      msm_combine_kernel<B><<<(unsigned)(g < cap ? g : cap), 256, 0, st>>>(mid.get(), n_lists.get(), unit_off.get(), partial.get(), buckets.get()); }
+      launch(ctx, msm_combine_kernel<B>, (unsigned)(g < cap ? g : cap), 256, 0, mid.get(), n_lists.get(), unit_off.get(), partial.get(), buckets.get()); }
     if ((max_entries >> chunk_log) > MSM_HEAVY_UNITS)  // e.g. the top window of a variable-base MSM, or a witness column that is mostly ones
-      msm_combine_heavy_kernel<B><<<(unsigned)(max_heavy < 296 ? max_heavy : 296), 256, 0, st>>>(heavy.get(), n_lists.get() + 1, unit_off.get(), partial.get(), buckets.get());
-    TB_LAUNCH_CHECK();
+      launch(ctx, msm_combine_heavy_kernel<B>, (unsigned)(max_heavy < 296 ? max_heavy : 296), 256, 0, heavy.get(), n_lists.get() + 1, unit_off.get(), partial.get(), buckets.get());
     ps.reset();
   }
   ps.reset(new ProfScope(ctx, PC_MSM_REDUCE));
@@ -402,9 +396,7 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
   Aff<B>* const aff_out = reinterpret_cast<Aff<B>*>(cfg_in.affine_out);
   if (wsep == 1 && NB < 64) {
     int threads = ((nt + 31) / 32) * 32;
-    msm_bucket_reduce_kernel<B><<<groups, threads, 0, st>>>(buckets.get(), NB, seg, nt, out, aff_out);
-    TB_LAUNCH_CHECK();
-    ctx->launches += 6;
+    launch(ctx, msm_bucket_reduce_kernel<B>, groups, threads, 0, buckets.get(), NB, seg, nt, out, aff_out);
     return;
   }
   if (wsep == 1) {
@@ -412,25 +404,18 @@ void msm_run(Ctx* ctx, const S* scalars, long long scalar_bstride, const Aff<B>*
     const int nl = (1 << s_log) + (1 << h_log), threads = 2 << s_log;
     TB_REQUIRE(threads <= 256, "fixed-base window too wide for the weighted-sum kernel (c <= 15)");
     DevBuf<Xyzz<B>> lines(ctx, (size_t)groups * nl);
-    msm_linesum_kernel<B><<<(unsigned)(((uint64_t)groups * nl * 16 + 127) / 128), 128, 0, st>>>(buckets.get(), NB, s_log, groups, lines.get());
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_linesum_kernel<B>, (unsigned)(((uint64_t)groups * nl * 16 + 127) / 128), 128, 0, buckets.get(), NB, s_log, groups, lines.get());
     const size_t smem = (size_t)threads * sizeof(Xyzz<B>);
     if (smem > 48 * 1024) {
       ctx->opt_in_smem(msm_weighted_kernel<B>, 128 * 1024);
     }
-    msm_weighted_kernel<B><<<groups, threads, smem, st>>>(lines.get(), s_log, h_log, out, aff_out);
-    TB_LAUNCH_CHECK();
-    ctx->launches += 7;
+    launch(ctx, msm_weighted_kernel<B>, groups, threads, smem, lines.get(), s_log, h_log, out, aff_out);
     return;
   }
   DevBuf<Xyzz<B>> seg_out(ctx, (size_t)groups * nt), win(ctx, groups);
-  msm_segsum_kernel<B><<<(groups * nt + 127) / 128, 128, 0, st>>>(buckets.get(), NB, seg, nt, groups, seg_out.get());
-  TB_LAUNCH_CHECK();
-  msm_window_kernel<B><<<groups, 256, 0, st>>>(seg_out.get(), nt, win.get());
-  TB_LAUNCH_CHECK();
-  msm_horner_kernel<B><<<(K + 31) / 32, 32, 0, st>>>(win.get(), wsep, c, K, out);
-  TB_LAUNCH_CHECK();
-  ctx->launches += 8;
+  launch(ctx, msm_segsum_kernel<B>, (groups * nt + 127) / 128, 128, 0, buckets.get(), NB, seg, nt, groups, seg_out.get());
+  launch(ctx, msm_window_kernel<B>, groups, 256, 0, seg_out.get(), nt, win.get());
+  launch(ctx, msm_horner_kernel<B>, (K + 31) / 32, 32, 0, win.get(), wsep, c, K, out);
 }
 
 template void msm_run<Fq, Fp>(Ctx*, const Fp*, long long, const Aff<Fq>*, long long, int, int, const MsmConfig&, Xyzz<Fq>*);
@@ -450,8 +435,7 @@ template <class B>
 void msm_build_tables(Ctx* ctx, const Aff<B>* bases, int N, int c, int windows, Aff<B>* table) {
   TB_CUDA(cudaMemcpyAsync(table, bases, (size_t)N * sizeof(Aff<B>), cudaMemcpyDeviceToDevice, ctx->stream));
   for (int w = 1; w < windows; ++w) {
-    msm_table_step_kernel<B><<<(N + 127) / 128, 128, 0, ctx->stream>>>(table + (size_t)(w - 1) * N, table + (size_t)w * N, N, c);
-    TB_LAUNCH_CHECK();
+    launch(ctx, msm_table_step_kernel<B>, (N + 127) / 128, 128, 0, table + (size_t)(w - 1) * N, table + (size_t)w * N, N, c);
   }
 }
 template void msm_build_tables<Fq>(Ctx*, const Aff<Fq>*, int, int, int, Aff<Fq>*);
@@ -463,8 +447,7 @@ __global__ void points_to_affine_kernel(const Xyzz<B>* __restrict__ acc, int K, 
   if (k < K) out[k] = acc[k].to_affine();
 }
 template <class B> void points_to_affine(Ctx* ctx, const Xyzz<B>* acc, int K, Aff<B>* out) {
-  points_to_affine_kernel<B><<<(K + 31) / 32, 32, 0, ctx->stream>>>(acc, K, out);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, points_to_affine_kernel<B>, (K + 31) / 32, 32, 0, acc, K, out);
 }
 template void points_to_affine<Fq>(Ctx*, const Xyzz<Fq>*, int, Aff<Fq>*);
 template void points_to_affine<Fp>(Ctx*, const Xyzz<Fp>*, int, Aff<Fp>*);

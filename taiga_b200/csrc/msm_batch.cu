@@ -408,12 +408,11 @@ static EncodeTiledFn encode_tiled_fn() {
 template <class B, bool FIRST>
 static void launch_round(Ctx* ctx, dim3 grid, size_t fwd_smem, size_t bwd_smem, const uint32_t* counts, int NB, int r, const uint32_t* entries, const Aff<B>* table, const B* in,
                          long long cap_in, B* out, long long cap_out, B* pre, B* tree, uint32_t* meta, uint2* eidx, const uint32_t* n_items, int R, uint32_t n_trees) {
-  cudaStream_t st = ctx->stream;
   ctx->opt_in_smem(msm_ba_fwd_kernel<B, FIRST>, fwd_smem);
   ctx->opt_in_smem(msm_ba_bwd_kernel<B, FIRST>, bwd_smem);
-  msm_ba_fwd_kernel<B, FIRST><<<grid, BA_THREADS, fwd_smem, st>>>(counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, eidx, n_items, R);
-  msm_ba_inv_kernel<B><<<(n_trees + 63) / 64, 64, 0, st>>>(tree, n_trees);
-  msm_ba_bwd_kernel<B, FIRST><<<grid, BA_THREADS, bwd_smem, st>>>(table, in, cap_in, out, cap_out, tree, meta, eidx, n_items, r, R);
+  launch(ctx, msm_ba_fwd_kernel<B, FIRST>, grid, BA_THREADS, fwd_smem, counts, NB, r, entries, table, in, cap_in, cap_out, pre, tree, meta, eidx, n_items, R);
+  launch(ctx, msm_ba_inv_kernel<B>, (n_trees + 63) / 64, 64, 0, tree, n_trees);
+  launch(ctx, msm_ba_bwd_kernel<B, FIRST>, grid, BA_THREADS, bwd_smem, table, in, cap_in, out, cap_out, tree, meta, eidx, n_items, r, R);
 }
 
 bool msm_batch_applicable(int N, int K, const MsmConfig& cfg, int c) {
@@ -427,7 +426,6 @@ template <class B, class S>
 void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<B>* table, int N, int K, int c, int W, int table_stride, const S* extras, int n_extra,
                        Xyzz<B>* buckets) {
   const int NB = 1 << (c - 1);
-  cudaStream_t st = ctx->stream;
   TB_REQUIRE(((uintptr_t)scalars & 15) == 0 && (sstride * (long long)sizeof(S)) % 16 == 0, "scalar vectors must be 16-byte aligned for TMA");
   const long long cap0 = (long long)(N + n_extra) * W;
   std::vector<long long> cap(1, cap0);
@@ -469,11 +467,10 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (cr != CUDA_SUCCESS) throw CudaError("cuTensorMapEncodeTiled failed for the scalar tensor (" + std::to_string((int)cr) + ")");
       const S* ex = extras ? extras + (long long)k0 * n_extra : nullptr;
-      if (c == 13) msm_sort_kernel<S, 13><<<kc, SORT_THREADS, sort_smem, st>>>(smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds);
-      else msm_sort_kernel<S, 0><<<kc, SORT_THREADS, sort_smem, st>>>(smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds);
-      TB_LAUNCH_CHECK(); ctx->launches++; }
+      if (c == 13) launch(ctx, msm_sort_kernel<S, 13>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds);
+      else launch(ctx, msm_sort_kernel<S, 0>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds); }
     { ProfScope ps(ctx, PC_MSM_ACCUM);
-      msm_ba_count_kernel<<<kc, BA_THREADS, 0, st>>>(counts.get(), NB, R, n_items.get());
+      launch(ctx, msm_ba_count_kernel, kc, BA_THREADS, 0, counts.get(), NB, R, n_items.get());
       for (int r = 0; r < R; ++r) {
         const B* in = (r & 1) ? itA.get() : itB.get();   // round r reads what round r-1 wrote (r = 0 reads the entries)
         B* out = (r & 1) ? itB.get() : itA.get();
@@ -482,11 +479,9 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
         const uint32_t n_trees = gx * (uint32_t)kc;
         (r == 0 ? launch_round<B, true> : launch_round<B, false>)(ctx, grid, fwd_smem, bwd_smem, counts.get(), NB, r, entries.get(), table, in, r == 0 ? cap0 : cap[r], out,
                                                                   cap[r + 1], out + cap[r + 1], tree.get(), meta.get(), eidx, n_items.get(), R, n_trees);
-        TB_LAUNCH_CHECK(); ctx->launches += 3;
       }
       const B* last = (R & 1) ? itA.get() : itB.get();
-      msm_ba_finish_kernel<B><<<dim3((NB + BA_THREADS - 1) / BA_THREADS, kc), BA_THREADS, fin_smem, st>>>(counts.get(), NB, R, last, cap[R], buckets + (size_t)k0 * NB);
-      TB_LAUNCH_CHECK(); ctx->launches++; }
+      launch(ctx, msm_ba_finish_kernel<B>, dim3((NB + BA_THREADS - 1) / BA_THREADS, kc), BA_THREADS, fin_smem, counts.get(), NB, R, last, cap[R], buckets + (size_t)k0 * NB); }
   }
 }
 

@@ -163,9 +163,7 @@ void ntt_run(Ctx* ctx, int logn, bool inverse, const F* in, F* out, F* scratch, 
     int R = 1 << a.r, T = 1 << a.logT;
     size_t smem = (size_t)R * (T == 1 ? 1 : T + 1) * 32;
     dim3 grid((1u << lanes_log) >> a.logT, batch, batch2);
-    ntt_pass_kernel<F><<<grid, NTT_THREADS, smem, ctx->stream>>>(src, dst, a);
-    TB_LAUNCH_CHECK();
-    ctx->launches++;
+    launch(ctx, ntt_pass_kernel<F>, grid, NTT_THREADS, smem, src, dst, a);
   }
 }
 
@@ -179,8 +177,7 @@ __global__ void ntt_hook_table_kernel(NttHook<F> h, TwiddleTables<F> tw, F* tabl
 }
 template <class F> void ntt_hook_table(Ctx* ctx, const NttHook<F>& hook, bool inverse, F* table, int n) {
   NttHook<F> h = hook; h.table = nullptr;
-  ntt_hook_table_kernel<F><<<(n + 255) / 256, 256, 0, ctx->stream>>>(h, inverse ? field_tables<F>(ctx).inv : field_tables<F>(ctx).fwd, table, n);
-  TB_LAUNCH_CHECK();
+  launch(ctx, ntt_hook_table_kernel<F>, (n + 255) / 256, 256, 0, h, inverse ? field_tables<F>(ctx).inv : field_tables<F>(ctx).fwd, table, n);
 }
 template void ntt_hook_table<Fp>(Ctx*, const NttHook<Fp>&, bool, Fp*, int);
 template void ntt_hook_table<Fq>(Ctx*, const NttHook<Fq>&, bool, Fq*, int);
@@ -206,13 +203,13 @@ void build_twiddles(Ctx* ctx) {
     TwiddleTables<F>& t = dir ? ft.inv : ft.fwd;
     TB_CUDA(cudaMalloc(&t.lo, n * sizeof(F)));
     TB_CUDA(cudaMalloc(&t.hi, n * sizeof(F)));
-    TB_CUDA(cudaMemcpy(t.lo, lo.data(), n * sizeof(F), cudaMemcpyHostToDevice));
-    TB_CUDA(cudaMemcpy(t.hi, hi.data(), n * sizeof(F), cudaMemcpyHostToDevice));
+    // on the context's stream, ahead of tw_fill_kernel which reads them (that stream does not wait for the legacy default stream)
+    TB_CUDA(cudaMemcpyAsync(t.lo, lo.data(), n * sizeof(F), cudaMemcpyHostToDevice, ctx->stream));
+    TB_CUDA(cudaMemcpyAsync(t.hi, hi.data(), n * sizeof(F), cudaMemcpyHostToDevice, ctx->stream));
     if (F::params_id() == 0) {  // circuit field only: 2 x 16 MB per context
       F* full = nullptr;
       TB_CUDA(cudaMalloc(&full, sizeof(F) << TW_FULL_LOG));
-      tw_fill_kernel<F><<<(1u << TW_FULL_LOG) / 256, 256>>>(t, full);
-      TB_CUDA(cudaGetLastError());
+      launch(ctx, tw_fill_kernel<F>, (1u << TW_FULL_LOG) / 256, 256, 0, t, full);
       TB_CUDA(cudaDeviceSynchronize());
       t.full = full; t.full_log = TW_FULL_LOG;
     }

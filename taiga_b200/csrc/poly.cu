@@ -14,11 +14,11 @@ __global__ void fe_convert_kernel(F* v, size_t n) {
 }
 template <class F> void fe_to_mont(Ctx* ctx, F* v, size_t n) {
   if (!n) return;
-  fe_convert_kernel<F, 1><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(v, n); TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, fe_convert_kernel<F, 1>, (unsigned)((n + 255) / 256), 256, 0, v, n);
 }
 template <class F> void fe_from_mont(Ctx* ctx, F* v, size_t n) {
   if (!n) return;
-  fe_convert_kernel<F, 0><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(v, n); TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, fe_convert_kernel<F, 0>, (unsigned)((n + 255) / 256), 256, 0, v, n);
 }
 template void fe_to_mont<Fp>(Ctx*, Fp*, size_t);
 template void fe_to_mont<Fq>(Ctx*, Fq*, size_t);
@@ -63,16 +63,14 @@ void exclusive_scan_u32(Ctx* ctx, const uint32_t* in, uint32_t* out, size_t n) {
   size_t nblocks = (n + SCAN_BLOCK - 1) / SCAN_BLOCK;
   if (nblocks == 0) { TB_CUDA(cudaMemsetAsync(out, 0, sizeof(uint32_t), ctx->stream)); return; }
   DevBuf<uint32_t> sums(ctx, nblocks);
-  scan_block_kernel<<<(unsigned)nblocks, SCAN_THREADS, 0, ctx->stream>>>(in, out, sums.get(), n);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, scan_block_kernel, (unsigned)nblocks, SCAN_THREADS, 0, in, out, sums.get(), n);
   if (nblocks == 1) {
     TB_CUDA(cudaMemcpyAsync(out + n, sums.get(), sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
     return;
   }
   DevBuf<uint32_t> offs(ctx, nblocks + 1);
   exclusive_scan_u32(ctx, sums.get(), offs.get(), nblocks);
-  scan_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(out, offs.get(), n);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, scan_add_kernel, (unsigned)((n + 255) / 256), 256, 0, out, offs.get(), n);
   TB_CUDA(cudaMemcpyAsync(out + n, offs.get() + nblocks, sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
 }
 

@@ -20,8 +20,7 @@ __global__ void poly_fma_kernel(Fp* out, long long out_stride, const Fp* s, long
 }
 void poly_fma(Ctx* c, Fp* out, long long out_stride, const Fp* s, long long s_stride, const Fp* in, long long in_stride, int n, int B) {
   ProfScope prof_scope(c, PC_POLY);
-  poly_fma_kernel<<<dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, c->stream>>>(out, out_stride, s, s_stride, in, in_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, poly_fma_kernel, dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, out, out_stride, s, s_stride, in, in_stride, n);
 }
 
 __global__ void poly_scale_kernel(Fp* out, long long out_stride, const Fp* s, long long s_stride, const Fp* a, long long a_stride, int n) {
@@ -30,8 +29,7 @@ __global__ void poly_scale_kernel(Fp* out, long long out_stride, const Fp* s, lo
   st_fe(out + (long long)b * out_stride + i, ld_fe(a + (long long)b * a_stride + i) * ld_fe(s + (long long)b * s_stride));
 }
 void poly_scale(Ctx* c, Fp* out, long long out_stride, const Fp* s, long long s_stride, const Fp* a, long long a_stride, int n, int B) {
-  poly_scale_kernel<<<dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, c->stream>>>(out, out_stride, s, s_stride, a, a_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, poly_scale_kernel, dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, out, out_stride, s, s_stride, a, a_stride, n);
 }
 
 __global__ void poly_copy_kernel(Fp* out, long long out_stride, const Fp* in, long long in_stride, int n) {
@@ -40,8 +38,7 @@ __global__ void poly_copy_kernel(Fp* out, long long out_stride, const Fp* in, lo
   st_fe(out + (long long)b * out_stride + i, ld_fe(in + (long long)b * in_stride + i));
 }
 void poly_copy(Ctx* c, Fp* out, long long out_stride, const Fp* in, long long in_stride, int n, int B) {
-  poly_copy_kernel<<<dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, c->stream>>>(out, out_stride, in, in_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, poly_copy_kernel, dim3((n + PO_THREADS - 1) / PO_THREADS, B), PO_THREADS, 0, out, out_stride, in, in_stride, n);
 }
 
 __global__ void poly_add_at_kernel(Fp* v, long long stride, int idx, const Fp* s, long long s_stride, int sign, int B) {
@@ -52,8 +49,7 @@ __global__ void poly_add_at_kernel(Fp* v, long long stride, int idx, const Fp* s
   *p = sign > 0 ? *p + sv : *p - sv;
 }
 void poly_add_at(Ctx* c, Fp* v, long long stride, int idx, const Fp* s, long long s_stride, int sign, int B) {
-  poly_add_at_kernel<<<(B + 31) / 32, 32, 0, c->stream>>>(v, stride, idx, s, s_stride, sign, B);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, poly_add_at_kernel, (B + 31) / 32, 32, 0, v, stride, idx, s, s_stride, sign, B);
 }
 
 // ---- block-wide sum of field elements (256 threads); result valid in thread 0
@@ -102,8 +98,7 @@ void poly_eval(Ctx* c, const EvalItem* d_items, int nitems, const Fp* points, lo
   ProfScope prof_scope(c, PC_POLY);
   if (nitems <= 0) return;
   TB_REQUIRE((n & (n - 1)) == 0, "poly_eval needs a power-of-two length");
-  poly_eval_kernel<<<dim3(nitems, B), PO_THREADS, 0, c->stream>>>(d_items, points, pt_stride, evals, ev_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, poly_eval_kernel, dim3(nitems, B), PO_THREADS, 0, d_items, points, pt_stride, evals, ev_stride, n);
 }
 
 __global__ void __launch_bounds__(PO_THREADS) inner_product_kernel(Fp* out, long long out_stride, const Fp* a, long long a_stride, const Fp* bv,
@@ -116,8 +111,7 @@ __global__ void __launch_bounds__(PO_THREADS) inner_product_kernel(Fp* out, long
   if (threadIdx.x == 0) out[(long long)b * out_stride] = acc;
 }
 void inner_product(Ctx* c, Fp* out, long long out_stride, const Fp* a, long long a_stride, const Fp* bvec, long long b_stride, int n, int B) {
-  inner_product_kernel<<<B, PO_THREADS, 0, c->stream>>>(out, out_stride, a, a_stride, bvec, b_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, inner_product_kernel, B, PO_THREADS, 0, out, out_stride, a, a_stride, bvec, b_stride, n);
 }
 
 __global__ void powers_kernel(Fp* out, long long out_stride, const Fp* x, long long x_stride, int n) {
@@ -133,8 +127,7 @@ __global__ void powers_kernel(Fp* out, long long out_stride, const Fp* x, long l
 }
 void powers(Ctx* c, Fp* out, long long out_stride, const Fp* x, long long x_stride, int n, int B) {
   int threads = (n + 15) / 16;
-  powers_kernel<<<dim3((threads + 127) / 128, B), 128, 0, c->stream>>>(out, out_stride, x, x_stride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, powers_kernel, dim3((threads + 127) / 128, B), 128, 0, out, out_stride, x, x_stride, n);
 }
 
 // ---------------------------------------------------------------- Kate division (suffix linear recurrence q_j = a_{j+1} + z q_{j+1})
@@ -206,13 +199,7 @@ void poly_kate_div(Ctx* c, Fp* out, long long out_stride, const Fp* in, long lon
   TB_REQUIRE((n & (n - 1)) == 0, "kate division needs a power-of-two length");
   const int cs = n >= KD_CLUSTER * KD_THREADS ? KD_CLUSTER : 1;
   TB_REQUIRE(n / (cs * (n / cs < KD_THREADS ? n / cs : KD_THREADS)) <= KD_MAX_M, "kate division: polynomial too long for one cluster");
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(B * cs)); cfg.blockDim = dim3(KD_THREADS); cfg.dynamicSmemBytes = 0; cfg.stream = c->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  TB_CUDA(cudaLaunchKernelEx(&cfg, kate_div_kernel, out, out_stride, in, in_stride, z, z_stride, n, cs));
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch_cluster(c, cs, kate_div_kernel, (unsigned)(B * cs), KD_THREADS, 0, out, out_stride, in, in_stride, z, z_stride, n, cs);
 }
 
 // ---------------------------------------------------------------- batch inversion (Montgomery trick, 16 elements per thread, zeros skipped)
@@ -236,8 +223,7 @@ __global__ void batch_inverse_kernel(Fp* v, size_t count) {
 void batch_inverse(Ctx* c, Fp* v, size_t count) {
   if (!count) return;
   size_t threads = (count + BI_CHUNK - 1) / BI_CHUNK;
-  batch_inverse_kernel<<<(unsigned)((threads + 63) / 64), 64, 0, c->stream>>>(v, count);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, batch_inverse_kernel, (unsigned)((threads + 63) / 64), 64, 0, v, count);
 }
 
 // ---------------------------------------------------------------- exclusive prefix product
@@ -267,8 +253,7 @@ __global__ void __launch_bounds__(PP_THREADS) prefix_product_kernel(Fp* out, con
 }
 void prefix_product(Ctx* c, Fp* out, const Fp* in, int n, int count) {
   TB_REQUIRE((n & (n - 1)) == 0 && out != in, "prefix_product arguments");
-  prefix_product_kernel<<<count, PP_THREADS, PP_THREADS * 32, c->stream>>>(out, in, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, prefix_product_kernel, count, PP_THREADS, PP_THREADS * 32, out, in, n);
 }
 
 // ---------------------------------------------------------------- per-proof scalar interpreter
@@ -297,8 +282,7 @@ __global__ void scalar_program_kernel(Fp* vars, long long stride, const ScalarIn
 }
 void scalar_program(Ctx* c, Fp* vars, long long stride, const ScalarInstr* d_prog, int ninstr, const Fp* d_consts, int B) {
   if (ninstr <= 0) return;
-  scalar_program_kernel<<<(B + 31) / 32, 32, 0, c->stream>>>(vars, stride, d_prog, ninstr, d_consts, B);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, scalar_program_kernel, (B + 31) / 32, 32, 0, vars, stride, d_prog, ninstr, d_consts, B);
 }
 
 }  // namespace tb

@@ -385,7 +385,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       off += instance_len[c];
     }
     fe_to_mont<Fp>(ctx, inst_vals.get(), (size_t)B * ni * n);
-    fill_const_kernel<<<(B * ni + 63) / 64, 64, 0, st>>>(blinds.get(), (size_t)B * ni, Fp::one());
+    launch(ctx, fill_const_kernel, (B * ni + 63) / 64, 64, 0, blinds.get(), (size_t)B * ni, Fp::one());
   }
   // ---- advice columns: upload, blinding rows, commit, iNTT
   Fp* const adv_polys = polys.get() + (size_t)O_ADV * n;
@@ -683,7 +683,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   WBuf<Fp> sfull = ws.buf<Fp>((size_t)B * n), cLR = ws.buf<Fp>((size_t)B * 2 * n), ex = ws.buf<Fp>((size_t)B * 4);
   WBuf<Xyzz<Fq>> accLR = ws.buf<Xyzz<Fq>>((size_t)B * 2);
   WBuf<Aff<Fq>> ptLR = ws.buf<Aff<Fq>>((size_t)B * 2);
-  fill_const_kernel<<<(unsigned)(((size_t)B * n + 255) / 256), 256, 0, st>>>(sfull.get(), (size_t)B * n, Fp::one());
+  launch(ctx, fill_const_kernel, (unsigned)(((size_t)B * n + 255) / 256), 256, 0, sfull.get(), (size_t)B * n, Fp::one());
   Prog round_prog;  // identical every round
   round_prog.op(S_INV, V_UINV, V_U); round_prog.op(S_MUL, V_T0, V_LR, V_UINV); round_prog.op(S_ADD, V_F, V_F, V_T0);
   round_prog.op(S_MUL, V_T0, V_RR, V_U); round_prog.op(S_ADD, V_F, V_F, V_T0);
@@ -691,20 +691,19 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   for (int j = 0; j < k; ++j) {
     int m = (int)(n >> j), half = m >> 1;
     { ProfScope fold_scope(ctx, PC_IPA_FOLD);
-      ipa_round_scalars_kernel<<<dim3((unsigned)((n + 255) / 256), B), 256, 0, st>>>(pprime.get(), sfull.get(), cLR.get(), (int)n, m); }
+      launch(ctx, ipa_round_scalars_kernel, dim3((unsigned)((n + 255) / 256), B), 256, 0, pprime.get(), sfull.get(), cLR.get(), (int)n, m); }
     inner_product(ctx, VP(V_VL), NV, pprime.get() + half, nn, bvec.get(), nn, half, B);
     inner_product(ctx, VP(V_VR), NV, pprime.get(), nn, bvec.get() + half, nn, half, B);
     prf_fill(ctx, seed, proof0, R_IPA_L, (uint32_t)j, VP(V_LR), NV, 1, 1, B);
     prf_fill(ctx, seed, proof0, R_IPA_R, (uint32_t)j, VP(V_RR), NV, 1, 1, B);
-    ipa_extras_kernel<<<(B + 31) / 32, 32, 0, st>>>(ex.get(), vars.get(), NV, V_LR, V_RR, V_VL, V_VR, V_Z, B);
+    launch(ctx, ipa_extras_kernel, (B + 31) / 32, 32, 0, ex.get(), vars.get(), NV, V_LR, V_RR, V_VL, V_VR, V_Z, B);
     // L_j, R_j = <cL | cR, g> + l_rand * w + (value * z) * u : one batched fixed-base MSM, K = 2 per proof
     srs.commit_xyzz(ctx, false, cLR.get(), nn, 2 * B, ex.get(), 2, accLR.get(), ptLR.get());
     tr.points(ptLR.get(), 2, 2, true);
     tr.squeeze(VP(V_U), NV, 1);
     scalar_program(ctx, vars.get(), NV, d_round, (int)round_prog.ins.size(), dconsts, B);
     { ProfScope fold_scope(ctx, PC_IPA_FOLD);
-      ipa_fold_kernel<<<dim3((unsigned)((n + 255) / 256), B), 256, 0, st>>>(pprime.get(), bvec.get(), sfull.get(), (int)n, half, vars.get(), NV, V_U, V_UINV); }
-    TB_LAUNCH_CHECK(); ctx->launches += 3;
+      launch(ctx, ipa_fold_kernel, dim3((unsigned)((n + 255) / 256), B), 256, 0, pprime.get(), bvec.get(), sfull.get(), (int)n, half, vars.get(), NV, V_U, V_UINV); }
   }
   poly_copy(ctx, VP(V_C), NV, pprime.get(), nn, 1, B);
   tr.scalars(VP(V_C), NV, 1, true);

@@ -306,8 +306,7 @@ static void q_launch(Ctx* c, const QPartList& pl, int nregs, const QData& d, int
   TB_REQUIRE(T >= 16 && T <= 128, "constraint program register file does not fit shared memory");
   while (T > d.n && T > 1) T >>= 1;
   const size_t smem = (size_t)(nregs + 2) * T * 32;
-  q_interp_kernel<<<dim3((d.n + T - 1) / T, B, pl.nparts), T, smem, c->stream>>>(pl, nregs, d);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, q_interp_kernel, dim3((d.n + T - 1) / T, B, pl.nparts), T, smem, pl, nregs, d);
 }
 void q_run(Ctx* c, const QProgram& prog, const QData& d, int B) {
   QPartList pl; memset(&pl, 0, sizeof(pl));

@@ -64,8 +64,7 @@ __global__ void __launch_bounds__(128) q_finish_kernel(QFinish f) {
 void q_finish(Ctx* c, const QFinish& f, int B) {
   ProfScope prof_scope(c, PC_QUOT_FINISH);
   c->work[PC_QUOT_FINISH] += (double)f.n * B * (3.0 * f.P + 6.0 * f.nsets + 16.0 * f.L + 2.0 * f.nparts + 8.0);   // permutation products, lookup terms, y folds
-  q_finish_kernel<<<dim3((f.n + 127) / 128, B), 128, 0, c->stream>>>(f);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, q_finish_kernel, dim3((f.n + 127) / 128, B), 128, 0, f);
 }
 
 // ---------------------------------------------------------------- extended_to_coeff, step B
@@ -90,8 +89,7 @@ __global__ void h_cross_kernel(const Fp* __restrict__ V, long long v_pstride, Fp
 }
 void h_cross(Ctx* c, const Fp* V, long long v_pstride, Fp* hcoef, long long h_pstride, int n, int R, int pieces, const Fp* d_wr_inv, int wr_step, Fp r_inv,
              Fp zeta_inv, int B) {
-  h_cross_kernel<<<dim3((n + 127) / 128, B), 128, 0, c->stream>>>(V, v_pstride, hcoef, h_pstride, n, R, pieces, d_wr_inv, wr_step, r_inv, zeta_inv);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, h_cross_kernel, dim3((n + 127) / 128, B), 128, 0, V, v_pstride, hcoef, h_pstride, n, R, pieces, d_wr_inv, wr_step, r_inv, zeta_inv);
 }
 
 // ---------------------------------------------------------------- low-degree part of the numerator (evaluated on every second sub-coset)
@@ -110,8 +108,7 @@ void q_combine(Ctx* c, const Fp* gate, int nparts, long long part_stride, const 
   ProfScope prof_scope(c, PC_QUOT_FINISH);
   QCombineArgs a; for (int p = 0; p < Q_MAX_PARTS; ++p) a.gexp[p] = p < nparts ? gexp[p] : 0;
   c->work[PC_QUOT_FINISH] += (double)n * B * nparts;
-  q_combine_kernel<<<dim3((n + 127) / 128, B), 128, 0, c->stream>>>(gate, nparts, part_stride, a, chal, chal_stride, ytab_slot, out, out_pstride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, q_combine_kernel, dim3((n + 127) / 128, B), 128, 0, gate, nparts, part_stride, a, chal, chal_stride, ytab_slot, out, out_pstride, n);
 }
 __global__ void q_lo_split_kernel(const Fp* __restrict__ coef, long long c_pstride, int m, Fp* __restrict__ r, long long r_pstride, Fp* __restrict__ q, long long q_pstride, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
@@ -122,8 +119,7 @@ __global__ void q_lo_split_kernel(const Fp* __restrict__ coef, long long c_pstri
   st_fe(r + (long long)b * r_pstride + i, run + ldg_fe(cb + i));
 }
 void q_lo_split(Ctx* c, const Fp* coef, long long c_pstride, int m, Fp* r, long long r_pstride, Fp* q, long long q_pstride, int n, int B) {
-  q_lo_split_kernel<<<dim3((n + 127) / 128, B), 128, 0, c->stream>>>(coef, c_pstride, m, r, r_pstride, q, q_pstride, n);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, q_lo_split_kernel, dim3((n + 127) / 128, B), 128, 0, coef, c_pstride, m, r, r_pstride, q, q_pstride, n);
 }
 __global__ void q_add_blocks_kernel(Fp* __restrict__ h, long long h_pstride, const Fp* __restrict__ q, long long q_pstride, int count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
@@ -133,8 +129,7 @@ __global__ void q_add_blocks_kernel(Fp* __restrict__ h, long long h_pstride, con
 }
 void q_add_blocks(Ctx* c, Fp* h, long long h_pstride, const Fp* q, long long q_pstride, int m, int n, int B) {
   const int count = m * n;
-  q_add_blocks_kernel<<<dim3((count + 255) / 256, B), 256, 0, c->stream>>>(h, h_pstride, q, q_pstride, count);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, q_add_blocks_kernel, dim3((count + 255) / 256, B), 256, 0, h, h_pstride, q, q_pstride, count);
 }
 
 // ---------------------------------------------------------------- grand products
@@ -162,8 +157,7 @@ __global__ void perm_fractions_kernel(PermFrac p) {
 }
 void perm_fractions(Ctx* c, const PermFrac& p, int B) {
   if (!p.nsets) return;
-  perm_fractions_kernel<<<dim3((p.n + 127) / 128, p.nsets, B), 128, 0, c->stream>>>(p);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, perm_fractions_kernel, dim3((p.n + 127) / 128, p.nsets, B), 128, 0, p);
 }
 
 __global__ void vec_mul_kernel(Fp* a, const Fp* b, size_t count) {
@@ -172,8 +166,7 @@ __global__ void vec_mul_kernel(Fp* a, const Fp* b, size_t count) {
 }
 void vec_mul(Ctx* c, Fp* a, const Fp* b, size_t count) {
   if (!count) return;
-  vec_mul_kernel<<<(unsigned)((count + 255) / 256), 256, 0, c->stream>>>(a, b, count);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, vec_mul_kernel, (unsigned)((count + 255) / 256), 256, 0, a, b, count);
 }
 
 __global__ void perm_carry_kernel(const Fp* z, long long pstride, int nsets, int n, int u, Fp* carries, int B) {
@@ -191,10 +184,8 @@ __global__ void perm_scale_kernel(Fp* z, long long pstride, int nsets, int n, co
 void perm_chain(Ctx* c, Fp* z, long long pstride, int nsets, int n, int u, int B) {
   if (nsets <= 1) return;
   DevBuf<Fp> carries(c, (size_t)B * nsets);
-  perm_carry_kernel<<<(B + 31) / 32, 32, 0, c->stream>>>(z, pstride, nsets, n, u, carries.get(), B);
-  TB_LAUNCH_CHECK();
-  perm_scale_kernel<<<dim3((n + 255) / 256, nsets, B), 256, 0, c->stream>>>(z, pstride, nsets, n, carries.get());
-  TB_LAUNCH_CHECK(); c->launches += 2;
+  launch(c, perm_carry_kernel, (B + 31) / 32, 32, 0, z, pstride, nsets, n, u, carries.get(), B);
+  launch(c, perm_scale_kernel, dim3((n + 255) / 256, nsets, B), 256, 0, z, pstride, nsets, n, carries.get());
 }
 
 __global__ void lookup_fractions_kernel(const Fp* A, const Fp* S, const Fp* Ap, const Fp* Sp, Fp* num, Fp* den, long long pstride, int n,
@@ -209,8 +200,7 @@ __global__ void lookup_fractions_kernel(const Fp* A, const Fp* S, const Fp* Ap, 
 void lookup_fractions(Ctx* c, const Fp* A, const Fp* S, const Fp* Ap, const Fp* Sp, Fp* num, Fp* den, long long pstride, int L, int n,
                       const Fp* chal, long long chal_stride, int beta_slot, int gamma_slot, int B) {
   if (!L) return;
-  lookup_fractions_kernel<<<dim3((n + 255) / 256, L, B), 256, 0, c->stream>>>(A, S, Ap, Sp, num, den, pstride, n, chal, chal_stride, beta_slot, gamma_slot);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, lookup_fractions_kernel, dim3((n + 255) / 256, L, B), 256, 0, A, S, Ap, Sp, num, den, pstride, n, chal, chal_stride, beta_slot, gamma_slot);
 }
 
 }  // namespace tb

@@ -145,23 +145,19 @@ void Transcripts::init(Ctx* c, int B_, uint32_t cap_, const Fp& vk_repr_canonica
   states = DevBuf<TrState>(c, B);
   proofs = DevBuf<uint8_t>(c, (size_t)B * cap);
   proofs.zero();
-  tr_init_kernel<<<(B + 31) / 32, 32, 0, c->stream>>>(states.get(), B, vk_repr_canonical);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, tr_init_kernel, (B + 31) / 32, 32, 0, states.get(), B, vk_repr_canonical);
 }
 void Transcripts::points(const Aff<Fq>* pts, long long stride, int count, bool write) {
   ProfScope prof_scope(ctx, PC_TRANSCRIPT);
-  tr_points_kernel<<<(B + 31) / 32, 32, 0, ctx->stream>>>(states.get(), proofs.get(), cap, B, pts, stride, count, write ? 1 : 0);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, tr_points_kernel, (B + 31) / 32, 32, 0, states.get(), proofs.get(), cap, B, pts, stride, count, write ? 1 : 0);
 }
 void Transcripts::scalars(const Fp* sc, long long stride, int count, bool write) {
   ProfScope prof_scope(ctx, PC_TRANSCRIPT);
-  tr_scalars_kernel<<<(B + 31) / 32, 32, 0, ctx->stream>>>(states.get(), proofs.get(), cap, B, sc, stride, count, write ? 1 : 0);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, tr_scalars_kernel, (B + 31) / 32, 32, 0, states.get(), proofs.get(), cap, B, sc, stride, count, write ? 1 : 0);
 }
 void Transcripts::squeeze(Fp* out, long long stride, int count) {
   ProfScope prof_scope(ctx, PC_TRANSCRIPT);
-  tr_squeeze_kernel<<<(B + 31) / 32, 32, 0, ctx->stream>>>(states.get(), B, out, stride, count);
-  TB_LAUNCH_CHECK(); ctx->launches++;
+  launch(ctx, tr_squeeze_kernel, (B + 31) / 32, 32, 0, states.get(), B, out, stride, count);
 }
 
 // ---------------------------------------------------------------- blinding PRF
@@ -190,8 +186,7 @@ void prf_fill(Ctx* c, const uint8_t* seed32, uint32_t proof0, uint32_t tag, uint
   if (count <= 0) return;
   SeedArg s; memcpy(s.w, seed32, 32);
   long long total = (long long)B * count;
-  prf_fill_kernel<<<(unsigned)((total + 127) / 128), 128, 0, c->stream>>>(s, proof0, tag, idx0, out, stride, elem_stride, count, B);
-  TB_LAUNCH_CHECK(); c->launches++;
+  launch(c, prf_fill_kernel, (unsigned)((total + 127) / 128), 128, 0, s, proof0, tag, idx0, out, stride, elem_stride, count, B);
 }
 
 }  // namespace tb

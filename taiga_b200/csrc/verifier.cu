@@ -351,11 +351,9 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
   d_ex.upload(extras.data(), extras.size());
   MsmConfig cfg;
   msm_run<Fq, Fp>(ctx, d_sc.get(), (long long)Mpad, d_pts.get(), (long long)Mpad, Mpad, K, cfg, acc_v.get());
-  verify_g_scalars_kernel<<<dim3((unsigned)((n + 255) / 256), K), 256, 0, st>>>(d_us.get(), d_cv.get(), d_gs.get(), kk, (int)n);
-  TB_LAUNCH_CHECK();
+  launch(ctx, verify_g_scalars_kernel, dim3((unsigned)((n + 255) / 256), K), 256, 0, d_us.get(), d_cv.get(), d_gs.get(), kk, (int)n);
   srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, d_ex.get(), 2, acc_g.get());
-  verify_final_kernel<<<(K + 31) / 32, 32, 0, st>>>(acc_v.get(), acc_g.get(), d_ok.get(), K);
-  TB_LAUNCH_CHECK(); ctx->launches += 2;
+  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K);
   std::vector<uint8_t> hok(K);
   d_ok.download(hok.data(), K); ctx->sync();
   for (int p = 0; p < K; ++p) ok_out[p] = (alive[p] && hok[p]) ? 1 : 0;
