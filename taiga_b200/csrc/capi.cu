@@ -30,8 +30,8 @@ tb_status tb_ctx_create(int device, tb_ctx** out) {
     TB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t thresh = UINT64_MAX;
     TB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thresh));
-    TB_CUDA(cudaMalloc(&ctx->c.d_msm_adds, sizeof(unsigned long long)));
-    TB_CUDA(cudaMemset(ctx->c.d_msm_adds, 0, sizeof(unsigned long long)));
+    ctx->c.d_msm_adds = DevMem<unsigned long long>(1);
+    TB_CUDA(cudaMemset(ctx->c.d_msm_adds.get(), 0, sizeof(unsigned long long)));
     build_twiddles<Fp>(&ctx->c);
     build_twiddles<Fq>(&ctx->c);
   } catch (const std::exception& e) {
@@ -46,10 +46,6 @@ tb_status tb_ctx_create(int device, tb_ctx** out) {
 void tb_ctx_destroy(tb_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->c.device);
-  cudaStreamSynchronize(ctx->c.stream);
-  free_twiddles<Fp>(&ctx->c); free_twiddles<Fq>(&ctx->c);
-  cudaFree(ctx->c.d_msm_adds);
-  cudaStreamDestroy(ctx->c.stream);
   delete ctx;
 }
 const char* tb_last_error(const tb_ctx* ctx) { return ctx ? ctx->c.last_error.c_str() : "null context"; }
@@ -88,8 +84,8 @@ tb_status tb_prof_work(tb_ctx* ctx, double* modmuls_out) {
   TB_API_BEGIN(ctx)
   ctx->c.sync();
   unsigned long long adds = 0;
-  TB_CUDA(cudaMemcpy(&adds, ctx->c.d_msm_adds, sizeof(adds), cudaMemcpyDeviceToHost));
-  TB_CUDA(cudaMemset(ctx->c.d_msm_adds, 0, sizeof(adds)));
+  TB_CUDA(cudaMemcpy(&adds, ctx->c.d_msm_adds.get(), sizeof(adds), cudaMemcpyDeviceToHost));
+  TB_CUDA(cudaMemset(ctx->c.d_msm_adds.get(), 0, sizeof(adds)));
   ctx->c.work[PC_MSM_ACCUM] += 6.4 * (double)adds;
   for (int i = 0; i < PC_COUNT; ++i) { modmuls_out[i] = ctx->c.work[i]; ctx->c.work[i] = 0; }
   TB_API_END(ctx)

@@ -13,14 +13,13 @@ namespace tb {
 enum PolyKind { PK_INST = 0, PK_ADV, PK_PZ, PK_LZ, PK_LPIN, PK_LPTAB, PK_FIXED, PK_SIG, PK_H, PK_RANDOM };
 struct PolyId { int kind, idx; bool operator<(const PolyId& o) const { return kind != o.kind ? kind < o.kind : idx < o.idx; } bool operator==(const PolyId& o) const { return kind == o.kind && idx == o.idx; } };
 struct QueryRef { PolyId poly; int rot; };
-struct WsBlock { void* p = nullptr; size_t bytes = 0; };
 // Scratch of one (context, batch size) pair: device blocks in request order and the small tables uploaded on first use.
 // A tb_pk may be shared by several contexts (= host threads); each gets its own workspace, and a second thread entering
 // with the SAME context and batch size while a call is in flight is refused (TB_ERR_INVALID) instead of corrupting it.
-struct ProveWs { std::vector<WsBlock> blocks; std::vector<void*> tables; std::vector<std::vector<uint8_t>> table_bytes; std::atomic<int> busy{0}; };
+struct ProveWs { std::vector<DevMem<uint8_t>> blocks, tables; std::vector<std::vector<uint8_t>> table_bytes; std::atomic<int> busy{0}; };
 
 struct Circuit {
-  Ctx* ctx; const Srs* srs;
+  const Srs* srs;
   // deep copy of the description
   uint32_t k, na, nf, ni, degree, bf, P, L, chunk, nsets, pieces; int ext_k, R; size_t n, usable;
   std::vector<tb_query> aq, fq, iq; std::vector<tb_column> perm;
@@ -28,10 +27,10 @@ struct Circuit {
   std::vector<std::vector<uint32_t>> lk_in, lk_tab;
   Fp vk_repr;  // canonical
   // device tables
-  Fp *fixed_vals = nullptr, *fixed_polys = nullptr, *fixed_cosets = nullptr, *sig_vals = nullptr, *sig_polys = nullptr, *sig_cosets = nullptr;
-  Fp *l0 = nullptr, *l_last = nullptr, *l_blind = nullptr, *consts = nullptr, *wr_inv = nullptr;
-  Fp* coset_pre = nullptr;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
-  int2* d_perm = nullptr;
+  DevMem<Fp> fixed_vals, fixed_polys, fixed_cosets, sig_vals, sig_polys, sig_cosets;
+  DevMem<Fp> l0, l_last, l_blind, consts, wr_inv;
+  DevMem<Fp> coset_pre;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
+  DevMem<int2> d_perm;
   QProgram prog_lookups;
   // gate programs in gate_nparts[big] parts, big = (batch size >= 8): small batches run more, shorter programs (latency), large
   // ones fewer (less duplicated work).  `gate_parts` holds the constraints evaluated on every sub-coset (all of them when the
@@ -59,31 +58,20 @@ struct Circuit {
     if (!slot) slot.reset(new ProveWs());
     return slot->busy.exchange(1) == 0 ? slot.get() : nullptr;
   }
-  // Out of device memory: frees the workspaces no call is using (other batch sizes, other contexts) and what the
-  // stream-ordered pool keeps cached, so that scratch kept for earlier calls does not make a new batch size fail.
-  void release_idle() const {
+  // Out of device memory on `device` (the calling context's): frees the workspaces no call is using (other batch sizes, other
+  // contexts) and what the stream-ordered pool keeps cached, so that scratch kept for earlier calls does not make a new batch size fail.
+  void release_idle(int device) const {
     TB_CUDA(cudaDeviceSynchronize());
     {
       std::lock_guard<std::mutex> lk(mu);
       for (auto it = ws.begin(); it != ws.end();) {
         if (it->second->busy.load() != 0) { ++it; continue; }
-        for (auto& b : it->second->blocks) cudaFree(b.p);
-        for (void* p : it->second->tables) cudaFree(p);
         it = ws.erase(it);
       }
     }
     cudaMemPool_t pool;
-    TB_CUDA(cudaDeviceGetDefaultMemPool(&pool, ctx->device));
+    TB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
     TB_CUDA(cudaMemPoolTrimTo(pool, 0));
-  }
-
-  ~Circuit() {
-    for (auto& kv : ws) { for (auto& b : kv.second->blocks) cudaFree(b.p); for (void* p : kv.second->tables) cudaFree(p); }
-    for (void* p : {(void*)fixed_vals, (void*)fixed_polys, (void*)fixed_cosets, (void*)sig_vals, (void*)sig_polys, (void*)sig_cosets, (void*)l0, (void*)l_last,
-                    (void*)l_blind, (void*)consts, (void*)wr_inv, (void*)coset_pre, (void*)d_perm, (void*)prog_lookups.dev})
-      if (p) cudaFree(p);
-    for (auto& progs : gate_parts) for (auto& qp : progs) if (qp.dev) cudaFree(qp.dev);
-    for (auto& progs : gate_parts_lo) for (auto& qp : progs) if (qp.dev) cudaFree(qp.dev);
   }
 };
 

@@ -1,5 +1,6 @@
 // Shared host-side plumbing for libtaiga_b200: context, error handling, stream-ordered device memory.
 #pragma once
+#include <algorithm>
 #include <cstdlib>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -26,6 +27,32 @@ struct ConstraintError : std::runtime_error { using std::runtime_error::runtime_
   } while (0)
 #define TB_REQUIRE(cond, msg) do { if (!(cond)) throw std::invalid_argument(std::string(msg) + " (" #cond ")"); } while (0)
 
+// Owner of one device allocation that outlives a call (SRS, proving key, context tables, workspaces): cudaMalloc / cudaFree,
+// which no stream orders, since such an allocation may outlive the context whose stream made it.  DevBuf is the stream-ordered
+// owner of per-call scratch.
+template <class T> struct DevMem {
+  DevMem() {}
+  explicit DevMem(size_t count) { TB_CUDA(try_alloc(count)); }
+  DevMem(const T* host, size_t count) : DevMem(count) { if (count) TB_CUDA(cudaMemcpy(p, host, count * sizeof(T), cudaMemcpyHostToDevice)); }
+  explicit DevMem(const std::vector<T>& v) : DevMem(v.data(), v.size()) {}
+  DevMem(const DevMem&) = delete; DevMem& operator=(const DevMem&) = delete;
+  DevMem(DevMem&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevMem& operator=(DevMem&& o) noexcept { if (this != &o) { reset(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; } return *this; }
+  ~DevMem() { reset(); }
+  void reset() { if (p) cudaFree(p); p = nullptr; n = 0; }
+  // frees what this holds, then allocates `count` elements (at least one); returns the error instead of throwing it
+  cudaError_t try_alloc(size_t count) {
+    reset();
+    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&p), std::max<size_t>(1, count) * sizeof(T));
+    if (e == cudaSuccess) n = count; else p = nullptr;
+    return e;
+  }
+  T* get() const { return p; }
+  size_t size() const { return n; }
+ private:
+  T* p = nullptr; size_t n = 0;
+};
+
 // NTT twiddle tables: powers of the 2^24-th root of unity, two-level (SURVEY E.3; tables are 2 x 128 KiB per
 // field and direction, L2 resident).  w_S^e = hi[e >> 12] * lo[e & 4095].
 constexpr int TW_LOG = 24;
@@ -36,7 +63,8 @@ template <class F> struct TwiddleTables { F* lo = nullptr; F* hi = nullptr; F* f
 constexpr int TW_FULL_LOG = 19;
 
 template <class F> struct FieldTables {
-  TwiddleTables<F> fwd, inv;
+  TwiddleTables<F> fwd, inv;   // what the kernels take by value: views of `mem`
+  DevMem<F> mem[2][3];         // [fwd, inv][lo, hi, full]
 };
 
 // kernel categories for the built-in CUDA-event profiler (bench.py's roofline / share-of-step numbers)
@@ -74,7 +102,15 @@ struct Ctx {
   // executed 255-bit Montgomery multiplications per kernel category (host-side accounting at every launch, for the integer-pipe
   // roofline of bench.py); the bucket additions of the batched MSM are counted on the device (they depend on the scalars)
   double work[PC_COUNT] = {0};
-  unsigned long long* d_msm_adds = nullptr;
+  DevMem<unsigned long long> d_msm_adds;
+  // tb_ctx_create may fail part way: every step skips what was never created
+  ~Ctx() {
+    if (stream) cudaStreamSynchronize(stream);
+    tw_fp = {}; tw_fq = {}; d_msm_adds.reset();
+    for (cudaEvent_t e : event_pool) cudaEventDestroy(e);
+    for (const ProfRec& r : prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
+    if (stream) cudaStreamDestroy(stream);
+  }
   cudaEvent_t get_event() {
     cudaEvent_t e;
     if (!event_pool.empty()) { e = event_pool.back(); event_pool.pop_back(); return e; }

@@ -19,7 +19,6 @@ void ntt_run(Ctx* ctx, int logn, bool inverse, const F* in, F* out, F* scratch, 
              long long out_bstride, const NttHook<F>* pre, const NttHook<F>* post, int batch2 = 1, long long in_b2stride = 0,
              long long out_b2stride = 0);  // scratch must hold batch2 * batch * 2^logn elements
 template <class F> void build_twiddles(Ctx* ctx);
-template <class F> void free_twiddles(Ctx* ctx);
 
 // ---------------------------------------------------------------- MSM (msm.cu)
 struct MsmConfig {

@@ -467,8 +467,8 @@ void msm_batch_buckets(Ctx* ctx, const S* scalars, long long sstride, const Aff<
                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (cr != CUDA_SUCCESS) throw CudaError("cuTensorMapEncodeTiled failed for the scalar tensor (" + std::to_string((int)cr) + ")");
       const S* ex = extras ? extras + (long long)k0 * n_extra : nullptr;
-      if (c == 13) launch(ctx, msm_sort_kernel<S, 13>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds);
-      else launch(ctx, msm_sort_kernel<S, 0>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds); }
+      if (c == 13) launch(ctx, msm_sort_kernel<S, 13>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds.get());
+      else launch(ctx, msm_sort_kernel<S, 0>, kc, SORT_THREADS, sort_smem, smap, ex, N, extras ? n_extra : 0, c, W, NB, table_stride, counts.get(), entries.get(), cap0, ctx->d_msm_adds.get()); }
     { ProfScope ps(ctx, PC_MSM_ACCUM);
       launch(ctx, msm_ba_count_kernel, kc, BA_THREADS, 0, counts.get(), NB, R, n_items.get());
       for (int r = 0; r < R; ++r) {

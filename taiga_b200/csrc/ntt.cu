@@ -201,29 +201,21 @@ void build_twiddles(Ctx* ctx) {
     lo[0] = F::one(); hi[0] = F::one();
     for (int i = 1; i < n; ++i) { lo[i] = lo[i - 1] * base; hi[i] = hi[i - 1] * step; }
     TwiddleTables<F>& t = dir ? ft.inv : ft.fwd;
-    TB_CUDA(cudaMalloc(&t.lo, n * sizeof(F)));
-    TB_CUDA(cudaMalloc(&t.hi, n * sizeof(F)));
+    DevMem<F>* mem = ft.mem[dir];
+    mem[0] = DevMem<F>(n); mem[1] = DevMem<F>(n);
+    t.lo = mem[0].get(); t.hi = mem[1].get();
     // on the context's stream, ahead of tw_fill_kernel which reads them (that stream does not wait for the legacy default stream)
     TB_CUDA(cudaMemcpyAsync(t.lo, lo.data(), n * sizeof(F), cudaMemcpyHostToDevice, ctx->stream));
     TB_CUDA(cudaMemcpyAsync(t.hi, hi.data(), n * sizeof(F), cudaMemcpyHostToDevice, ctx->stream));
     if (F::params_id() == 0) {  // circuit field only: 2 x 16 MB per context
-      F* full = nullptr;
-      TB_CUDA(cudaMalloc(&full, sizeof(F) << TW_FULL_LOG));
-      launch(ctx, tw_fill_kernel<F>, (1u << TW_FULL_LOG) / 256, 256, 0, t, full);
+      mem[2] = DevMem<F>(size_t(1) << TW_FULL_LOG);
+      launch(ctx, tw_fill_kernel<F>, (1u << TW_FULL_LOG) / 256, 256, 0, t, mem[2].get());
       TB_CUDA(cudaDeviceSynchronize());
-      t.full = full; t.full_log = TW_FULL_LOG;
+      t.full = mem[2].get(); t.full_log = TW_FULL_LOG;
     }
   }
 }
 template void build_twiddles<Fp>(Ctx*);
 template void build_twiddles<Fq>(Ctx*);
-
-template <class F>
-void free_twiddles(Ctx* ctx) {
-  FieldTables<F>& ft = field_tables<F>(ctx);
-  cudaFree(ft.fwd.lo); cudaFree(ft.fwd.hi); cudaFree(ft.inv.lo); cudaFree(ft.inv.hi); cudaFree(ft.fwd.full); cudaFree(ft.inv.full);
-}
-template void free_twiddles<Fp>(Ctx*);
-template void free_twiddles<Fq>(Ctx*);
 
 }  // namespace tb

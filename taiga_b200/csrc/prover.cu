@@ -17,26 +17,18 @@
 
 namespace tb {
 
-template <class T> static T* dev_upload(const std::vector<T>& v) {
-  T* p = nullptr;
-  TB_CUDA(cudaMalloc(&p, std::max<size_t>(1, v.size()) * sizeof(T)));
-  if (!v.empty()) TB_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  return p;
-}
-static Fp* dev_alloc_fp(size_t count) { Fp* p = nullptr; TB_CUDA(cudaMalloc(&p, std::max<size_t>(1, count) * sizeof(Fp))); return p; }
-
 static NttHook<Fp> coset_hook(const Circuit& C, int k1, bool inverse) {
   NttHook<Fp> h; h.use_const = 0; h.mod_bits = C.ext_k; h.k = (uint32_t)k1;
-  if (!inverse) { h.use_zeta = 1; h.z1 = C.zeta; h.z2 = C.zeta.sqr(); h.table = C.coset_pre + (size_t)k1 * C.n; }
+  if (!inverse) { h.use_zeta = 1; h.z1 = C.zeta; h.z2 = C.zeta.sqr(); h.table = C.coset_pre.get() + (size_t)k1 * C.n; }
   else { h.use_zeta = 0; h.z1 = Fp::one(); h.z2 = Fp::one(); }
   return h;
 }
 // polys [count][n] -> cosets [count][R][n] (sub-coset major)
-static void to_cosets(const Circuit& C, const Fp* polys, Fp* cosets, Fp* scratch, int count) {
+static void to_cosets(Ctx* ctx, const Circuit& C, const Fp* polys, Fp* cosets, Fp* scratch, int count) {
   if (!count) return;
   for (int k1 = 0; k1 < C.R; ++k1) {
     NttHook<Fp> h = coset_hook(C, k1, false);
-    ntt_run<Fp>(C.ctx, (int)C.k, false, polys, cosets + (size_t)k1 * C.n, scratch, count, (long long)C.n, (long long)C.R * C.n, &h, nullptr);
+    ntt_run<Fp>(ctx, (int)C.k, false, polys, cosets + (size_t)k1 * C.n, scratch, count, (long long)C.n, (long long)C.R * C.n, &h, nullptr);
   }
 }
 
@@ -45,7 +37,7 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   TB_REQUIRE(cs->cs_degree >= 3 && cs->num_perm_columns <= 16 * (cs->cs_degree - 2), "unsupported constraint system shape");
   std::unique_ptr<Circuit> Cp(new Circuit());
   Circuit& C = *Cp;
-  C.ctx = ctx; C.srs = srs;
+  C.srs = srs;
   C.k = cs->k; C.n = size_t(1) << C.k; C.na = cs->num_advice; C.nf = cs->num_fixed; C.ni = cs->num_instance; C.degree = cs->cs_degree; C.bf = cs->blinding_factors;
   TB_REQUIRE(C.n > C.bf + 2, "too few rows");
   C.usable = C.n - (C.bf + 1);
@@ -104,29 +96,29 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   { Fp zn = C.zeta.pow_u64(C.n), step = w_ext.pow_u64(C.n), cur = zn;
     for (int k1 = 0; k1 < C.R; ++k1) { C.t_inv.push_back((cur - Fp::one()).inv()); cur = cur * step; }
     std::vector<Fp> wr(C.R); Fp wri = step.inv(); wr[0] = Fp::one(); for (int e = 1; e < C.R; ++e) wr[e] = wr[e - 1] * wri;
-    C.wr_inv = dev_upload(wr); }
+    C.wr_inv = DevMem<Fp>(wr); }
 
   size_t n = C.n;
   // constants -> Montgomery
   { std::vector<Fp> cm(C.nconsts);
     for (uint32_t i = 0; i < C.nconsts; ++i) { Fp v; memcpy(v.l, C.consts_bytes.data() + 32 * i, 32); cm[i] = v.to_mont(); }
-    C.consts = dev_upload(cm); }
-  { std::vector<int2> pc; for (auto& c : C.perm) pc.push_back(make_int2((int)c.kind, (int)c.index)); C.d_perm = dev_upload(pc); }
+    C.consts = DevMem<Fp>(cm); }
+  { std::vector<int2> pc; for (auto& c : C.perm) pc.push_back(make_int2((int)c.kind, (int)c.index)); C.d_perm = DevMem<int2>(pc); }
 
   { // per-element factors of the forward coset hooks (one multiplication per coefficient instead of up to two and a table walk);
     // ntt_hook_table computes them from the hook without its table
-    C.coset_pre = dev_alloc_fp((size_t)C.R * n);
-    for (int k1 = 0; k1 < C.R; ++k1) { NttHook<Fp> h = coset_hook(C, k1, false); ntt_hook_table<Fp>(ctx, h, false, C.coset_pre + (size_t)k1 * n, (int)n); }
+    C.coset_pre = DevMem<Fp>((size_t)C.R * n);
+    for (int k1 = 0; k1 < C.R; ++k1) { NttHook<Fp> h = coset_hook(C, k1, false); ntt_hook_table<Fp>(ctx, h, false, C.coset_pre.get() + (size_t)k1 * n, (int)n); }
     ctx->sync();
   }
   DevBuf<Fp> scratch(ctx, std::max<size_t>(3, std::max<size_t>(C.nf, C.P)) * n);
-  auto load_cols = [&](const uint8_t* src, size_t cnt, Fp*& vals, Fp*& polys, Fp*& cosets) {
-    vals = dev_alloc_fp(cnt * n); polys = dev_alloc_fp(cnt * n); cosets = dev_alloc_fp(cnt * C.R * n);
+  auto load_cols = [&](const uint8_t* src, size_t cnt, DevMem<Fp>& vals, DevMem<Fp>& polys, DevMem<Fp>& cosets) {
+    vals = DevMem<Fp>(cnt * n); polys = DevMem<Fp>(cnt * n); cosets = DevMem<Fp>(cnt * C.R * n);
     if (!cnt) return;
-    TB_CUDA(cudaMemcpyAsync(vals, src, cnt * n * 32, cudaMemcpyHostToDevice, ctx->stream));
-    fe_to_mont<Fp>(ctx, vals, cnt * n);
-    ntt_run<Fp>(ctx, (int)C.k, true, vals, polys, scratch.get(), (int)cnt, (long long)n, (long long)n, nullptr, nullptr);
-    to_cosets(C, polys, cosets, scratch.get(), (int)cnt);
+    TB_CUDA(cudaMemcpyAsync(vals.get(), src, cnt * n * 32, cudaMemcpyHostToDevice, ctx->stream));
+    fe_to_mont<Fp>(ctx, vals.get(), cnt * n);
+    ntt_run<Fp>(ctx, (int)C.k, true, vals.get(), polys.get(), scratch.get(), (int)cnt, (long long)n, (long long)n, nullptr, nullptr);
+    to_cosets(ctx, C, polys.get(), cosets.get(), scratch.get(), (int)cnt);
   };
   load_cols(fixed, C.nf, C.fixed_vals, C.fixed_polys, C.fixed_cosets);
   load_cols(sigma, C.P, C.sig_vals, C.sig_polys, C.sig_cosets);
@@ -137,12 +129,12 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
     DevBuf<Fp> lv(ctx, 3 * n), lp(ctx, 3 * n), lc(ctx, 3 * (size_t)C.R * n);
     lv.upload(lag.data(), 3 * n);
     ntt_run<Fp>(ctx, (int)C.k, true, lv.get(), lp.get(), scratch.get(), 3, (long long)n, (long long)n, nullptr, nullptr);
-    to_cosets(C, lp.get(), lc.get(), scratch.get(), 3);
-    C.l0 = dev_alloc_fp((size_t)C.R * n); C.l_last = dev_alloc_fp((size_t)C.R * n); C.l_blind = dev_alloc_fp((size_t)C.R * n);
+    to_cosets(ctx, C, lp.get(), lc.get(), scratch.get(), 3);
+    C.l0 = DevMem<Fp>((size_t)C.R * n); C.l_last = DevMem<Fp>((size_t)C.R * n); C.l_blind = DevMem<Fp>((size_t)C.R * n);
     size_t sz = (size_t)C.R * n * sizeof(Fp);
-    TB_CUDA(cudaMemcpyAsync(C.l0, lc.get(), sz, cudaMemcpyDeviceToDevice, ctx->stream));
-    TB_CUDA(cudaMemcpyAsync(C.l_last, lc.get() + (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
-    TB_CUDA(cudaMemcpyAsync(C.l_blind, lc.get() + 2 * (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
+    TB_CUDA(cudaMemcpyAsync(C.l0.get(), lc.get(), sz, cudaMemcpyDeviceToDevice, ctx->stream));
+    TB_CUDA(cudaMemcpyAsync(C.l_last.get(), lc.get() + (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
+    TB_CUDA(cudaMemcpyAsync(C.l_blind.get(), lc.get() + 2 * (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->sync(); }
 
   // expression programs (descriptor rebuilt from the deep copy so pointers stay valid)
@@ -159,9 +151,7 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
       q_compile_gates_split(&d, all, 1, &t_all); q_compile_gates_split(&d, lo, 1, &t_lo);
       C.split = tb_tune("TB_Q_SPLIT", 1) != 0 && C.R >= 4 && !lo.empty() && !hi.empty() && t_lo[0].ninstr * 10 >= t_all[0].ninstr * 3;
       if (getenv("TB_DEBUG")) fprintf(stderr, "[tb] circuit k=%u degree=%u: %u constraints, %zu of degree <= %d (%d of %d instructions): split %s\n", C.k, C.degree, cs->num_constraints,
-                                      lo.size(), C.R / 2, t_lo[0].ninstr, t_all[0].ninstr, C.split ? "on" : "off");
-      for (auto& qp : t_all) if (qp.dev) cudaFree(qp.dev);
-      for (auto& qp : t_lo) if (qp.dev) cudaFree(qp.dev); }
+                                      lo.size(), C.R / 2, t_lo[0].ninstr, t_all[0].ninstr, C.split ? "on" : "off"); }
     for (int big = 0; big < 2; ++big) {
       q_compile_gates_split(&d, C.split ? hi : all, Circuit::gate_nparts[big], &C.gate_parts[big]);
       if (C.split) q_compile_gates_split(&d, lo, Circuit::gate_nparts[big], &C.gate_parts_lo[big]);
@@ -278,19 +268,16 @@ template <class T> struct WBuf {
   void zero() { TB_CUDA(cudaMemsetAsync(p, 0, n * sizeof(T), ctx->stream)); }
 };
 struct WsAlloc {
-  Ctx* ctx; const Circuit& C; std::vector<WsBlock>& blocks; size_t cur = 0;
-  void* device_malloc(size_t bytes) {
-    void* p = nullptr;
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); C.release_idle(); e = cudaMalloc(&p, bytes); }
-    TB_CUDA(e);
-    return p;
-  }
+  Ctx* ctx; const Circuit& C; std::vector<DevMem<uint8_t>>& blocks; size_t cur = 0;
   template <class T> WBuf<T> buf(size_t count) {
     size_t bytes = std::max<size_t>(1, count) * sizeof(T);
-    if (cur == blocks.size()) { WsBlock b; b.bytes = bytes; b.p = device_malloc(bytes); blocks.push_back(b); }
-    else if (blocks[cur].bytes < bytes) { cudaFree(blocks[cur].p); blocks[cur].p = nullptr; blocks[cur].bytes = 0; blocks[cur].p = device_malloc(bytes); blocks[cur].bytes = bytes; }
-    WBuf<T> w; w.p = reinterpret_cast<T*>(blocks[cur].p); w.n = count; w.ctx = ctx; ++cur;
+    if (cur == blocks.size()) blocks.emplace_back();
+    if (blocks[cur].size() < bytes) {   // try_alloc frees the smaller block first
+      cudaError_t e = blocks[cur].try_alloc(bytes);
+      if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); C.release_idle(ctx->device); e = blocks[cur].try_alloc(bytes); }
+      TB_CUDA(e);
+    }
+    WBuf<T> w; w.p = reinterpret_cast<T*>(blocks[cur].get()); w.n = count; w.ctx = ctx; ++cur;
     return w;
   }
 };
@@ -313,7 +300,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   ProveWs& pws = *claimed;
   struct BusyGuard { std::atomic<int>& f; ~BusyGuard() { f.store(0); } } guard{pws.busy};
   WsAlloc ws{ctx, C, pws.blocks};
-  std::vector<void*>& tables = pws.tables;
+  std::vector<DevMem<uint8_t>>& tables = pws.tables;
   size_t table_cur = 0;
   // uploads a small host table once per (circuit, context, B); later calls reuse the device copy.  The contents follow from the
   // circuit and B alone; they are still compared with what was uploaded (a cheap guard should a table come to depend on anything
@@ -321,18 +308,18 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   auto cached_upload = [&](const void* host, size_t bytes) -> void* {
     const uint8_t* hb = static_cast<const uint8_t*>(host);
     if (table_cur == tables.size()) {
-      void* d = nullptr; TB_CUDA(cudaMalloc(&d, std::max<size_t>(16, bytes)));
-      TB_CUDA(cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice));
-      tables.push_back(d); pws.table_bytes.emplace_back(hb, hb + bytes);
+      tables.emplace_back(std::max<size_t>(16, bytes));
+      TB_CUDA(cudaMemcpy(tables.back().get(), host, bytes, cudaMemcpyHostToDevice));
+      pws.table_bytes.emplace_back(hb, hb + bytes);
     } else {
       std::vector<uint8_t>& old = pws.table_bytes[table_cur];
       if (old.size() != bytes || memcmp(old.data(), host, bytes) != 0) {
-        if (old.size() < bytes) { cudaFree(tables[table_cur]); TB_CUDA(cudaMalloc(&tables[table_cur], bytes)); }
+        if (old.size() < bytes) tables[table_cur] = DevMem<uint8_t>(bytes);
         old.assign(hb, hb + bytes);
-        TB_CUDA(cudaMemcpyAsync(tables[table_cur], old.data(), bytes, cudaMemcpyHostToDevice, st));
+        TB_CUDA(cudaMemcpyAsync(tables[table_cur].get(), old.data(), bytes, cudaMemcpyHostToDevice, st));
       }
     }
-    return tables[table_cur++];
+    return tables[table_cur++].get();
   };
 
   // ---- per-proof scalar variables
@@ -410,11 +397,11 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   WBuf<Fp> lptab; lptab.p = lperm.get() + (size_t)B * L * n; lptab.n = (size_t)B * L1 * n; lptab.ctx = ctx;   // adjacent: one commitment call
   Fp* const lpin_polys = polys.get() + (size_t)O_LPIN * n; Fp* const lptab_polys = polys.get() + (size_t)O_LPTAB * n;
   QData qd; memset(&qd, 0, sizeof(qd));
-  qd.consts = C.consts; qd.chal = vars.get(); qd.chal_stride = NV; qd.y_slot = V_Y; qd.theta_slot = V_THETA; qd.ytab_slot = V_YTAB;
+  qd.consts = C.consts.get(); qd.chal = vars.get(); qd.chal_stride = NV; qd.y_slot = V_Y; qd.theta_slot = V_THETA; qd.ytab_slot = V_YTAB;
   qd.n = (int)n; qd.lk_pstride = (long long)L1 * nn;
   if (L) {
     qd.adv = adv_vals.get(); qd.adv_pstride = (long long)na * nn; qd.inst = inst_vals.get(); qd.inst_pstride = (long long)ni1 * nn;
-    qd.fix = C.fixed_vals; qd.R = 1; qd.k1 = 0; qd.gate_out = nullptr; qd.lkA = lkA.get(); qd.lkS = lkS.get();
+    qd.fix = C.fixed_vals.get(); qd.R = 1; qd.k1 = 0; qd.gate_out = nullptr; qd.lkA = lkA.get(); qd.lkS = lkS.get();
     q_run(ctx, C.prog_lookups, qd, B);
     WBuf<Fp> keysA = ws.buf<Fp>((size_t)B * L * n), keysS = ws.buf<Fp>((size_t)B * L * n), left = ws.buf<Fp>((size_t)B * L * n);
     lookup_keys(ctx, keysA.get(), lkA.get(), (int)n, (int)C.usable, B * L);
@@ -449,8 +436,8 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   Fp* const gz_lk = gz.get() + (size_t)B * nsets * n;   // lookup Z vectors directly after the permutation Z vectors: one commitment call
   if (nsets) {
     PermFrac pf; memset(&pf, 0, sizeof(pf));
-    pf.adv = adv_vals.get(); pf.adv_pstride = (long long)na * nn; pf.inst = inst_vals.get(); pf.inst_pstride = (long long)ni1 * nn; pf.fix = C.fixed_vals;
-    pf.sig = C.sig_vals; pf.perm_cols = C.d_perm; pf.P = P; pf.chunk = C.chunk; pf.nsets = nsets; pf.chal = vars.get(); pf.chal_stride = NV;
+    pf.adv = adv_vals.get(); pf.adv_pstride = (long long)na * nn; pf.inst = inst_vals.get(); pf.inst_pstride = (long long)ni1 * nn; pf.fix = C.fixed_vals.get();
+    pf.sig = C.sig_vals.get(); pf.perm_cols = C.d_perm.get(); pf.P = P; pf.chunk = C.chunk; pf.nsets = nsets; pf.chal = vars.get(); pf.chal_stride = NV;
     pf.beta_slot = V_BETA; pf.gamma_slot = V_GAMMA; pf.delta = C.delta; pf.omega = C.omega; memcpy(pf.delta_c0, C.delta_c0, sizeof(pf.delta_c0));
     pf.tw = ctx->tw_fp.fwd; pf.num = gnum.get(); pf.den = gden.get(); pf.pstride = (long long)nsets * nn; pf.n = (int)n; pf.k = k;
     perm_fractions(ctx, pf, B);
@@ -524,7 +511,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
         NttHook<Fp> h = coset_hook(C, k1, false);
         ntt_run<Fp>(ctx, k, false, polys.get(), ck, scratch.get(), B * NC, nn, nn, &h, nullptr);
         qd.adv = ck + (size_t)O_ADV * n; qd.adv_pstride = PS; qd.inst = ck + (size_t)O_INST * n; qd.inst_pstride = PS;
-        qd.fix = C.fixed_cosets; qd.R = R; qd.k1 = k1; qd.lkA = c_lkA.get(); qd.lkS = c_lkS.get();
+        qd.fix = C.fixed_cosets.get(); qd.R = R; qd.k1 = k1; qd.lkA = c_lkA.get(); qd.lkS = c_lkS.get();
         qd.gate_out = gate.get(); qd.gate_pstride = nn;
         q_run_parts(ctx, *lprogs, qd, (long long)B * nn, B);
         q_combine(ctx, gate.get(), (int)lprogs->size(), (long long)B * nn, gexp, vars.get(), NV, V_YTAB, elo.get() + (size_t)kq * n, (long long)Rlo * nn, (int)n, B);
@@ -533,7 +520,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
         NttHook<Fp> h = coset_hook(C, 2 * kq, true);
         ntt_run<Fp>(ctx, k, true, elo.get() + (size_t)kq * n, vlo.get() + (size_t)kq * n, scratch.get(), B, (long long)Rlo * nn, (long long)Rlo * nn, nullptr, &h);
       }
-      h_cross(ctx, vlo.get(), (long long)Rlo * nn, clo.get(), (long long)Rlo * nn, (int)n, Rlo, Rlo, C.wr_inv, 2, Fp::from_u32((uint32_t)Rlo).inv(), C.zeta.sqr(), B);
+      h_cross(ctx, vlo.get(), (long long)Rlo * nn, clo.get(), (long long)Rlo * nn, (int)n, Rlo, Rlo, C.wr_inv.get(), 2, Fp::from_u32((uint32_t)Rlo).inv(), C.zeta.sqr(), B);
       q_lo_split(ctx, clo.get(), (long long)Rlo * nn, Rlo, rlo_poly.get(), nn, qlo.get(), (long long)Rlo * nn, (int)n, B);
     }
     int gexp_hi[Q_MAX_PARTS] = {0};
@@ -547,7 +534,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       Fp* const c_adv = ck + (size_t)O_ADV * n; Fp* const c_inst = ck + (size_t)O_INST * n; Fp* const c_pz = ck + (size_t)O_PZ * n;
       Fp* const c_lz = ck + (size_t)O_LZ * n; Fp* const c_lpin = ck + (size_t)O_LPIN * n; Fp* const c_lptab = ck + (size_t)O_LPTAB * n;
       qd.adv = c_adv; qd.adv_pstride = PS; qd.inst = c_inst; qd.inst_pstride = PS;
-      qd.fix = C.fixed_cosets; qd.R = R; qd.k1 = k1; qd.lkA = c_lkA.get(); qd.lkS = c_lkS.get();
+      qd.fix = C.fixed_cosets.get(); qd.R = R; qd.k1 = k1; qd.lkA = c_lkA.get(); qd.lkS = c_lkS.get();
       qd.gate_out = gate.get(); qd.gate_pstride = nn;
       q_run_parts(ctx, gprogs, qd, (long long)B * nn, B);
       if (L) { qd.gate_out = nullptr; q_run(ctx, C.prog_lookups, qd, B); }
@@ -555,9 +542,9 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       f.gate = gate.get(); f.nparts = (int)gprogs.size(); f.gate_part_stride = (long long)B * nn; f.ytab_slot = V_YTAB; memcpy(f.gexp, gexp_hi, sizeof(gexp_hi));
       f.rlo = C.split ? rlo_coset.get() : nullptr; f.rlo_pstride = nn;
       f.adv = c_adv; f.adv_pstride = PS; f.inst = c_inst; f.inst_pstride = PS;
-      f.fix = C.fixed_cosets; f.sig = C.sig_cosets; f.R = R; f.k1 = k1; f.l0 = C.l0; f.l_last = C.l_last; f.l_blind = C.l_blind;
+      f.fix = C.fixed_cosets.get(); f.sig = C.sig_cosets.get(); f.R = R; f.k1 = k1; f.l0 = C.l0.get(); f.l_last = C.l_last.get(); f.l_blind = C.l_blind.get();
       f.pz = c_pz; f.pz_pstride = PS; f.lz = c_lz; f.lpin = c_lpin; f.lptab = c_lptab; f.lk_pstride = PS; f.lkc_pstride = (long long)L1 * nn;
-      f.lkA = c_lkA.get(); f.lkS = c_lkS.get(); f.perm_cols = C.d_perm; f.P = P; f.chunk = C.chunk; f.nsets = nsets; f.L = L; f.bf = bf;
+      f.lkA = c_lkA.get(); f.lkS = c_lkS.get(); f.perm_cols = C.d_perm.get(); f.P = P; f.chunk = C.chunk; f.nsets = nsets; f.L = L; f.bf = bf;
       f.chal = vars.get(); f.chal_stride = NV; f.y_slot = V_Y; f.beta_slot = V_BETA; f.gamma_slot = V_GAMMA;
       f.delta = C.delta; f.zeta = C.zeta; f.t_inv = C.t_inv[k1]; memcpy(f.delta_c0, C.delta_c0, sizeof(f.delta_c0)); f.tw = ctx->tw_fp.fwd;
       f.ext_k = C.ext_k; f.k = k; f.out = hext.get(); f.out_pstride = (long long)R * nn; f.n = (int)n;
@@ -568,7 +555,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       NttHook<Fp> h = coset_hook(C, k1, true);
       ntt_run<Fp>(ctx, k, true, hext.get() + (size_t)k1 * n, V.get() + (size_t)k1 * n, scratch.get(), B, (long long)R * nn, (long long)R * nn, nullptr, &h);
     }
-    h_cross(ctx, V.get(), (long long)R * nn, hcoef.get(), (long long)C.pieces * nn, (int)n, R, (int)C.pieces, C.wr_inv, 1, C.r_inv, C.zeta.sqr(), B);
+    h_cross(ctx, V.get(), (long long)R * nn, hcoef.get(), (long long)C.pieces * nn, (int)n, R, (int)C.pieces, C.wr_inv.get(), 1, C.r_inv, C.zeta.sqr(), B);
     if (C.split) q_add_blocks(ctx, hcoef.get(), (long long)C.pieces * nn, qlo.get(), (long long)Rlo * nn, Rlo - 1, (int)n, B);   // + H_lo div (X^n - 1)
   }
   prf_fill(ctx, seed, proof0, R_H_BLIND, 0, VP(V_H_BLINDS), NV, 1, (int)C.pieces, B);
@@ -603,8 +590,8 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       case PK_LZ: return {lz_polys + (size_t)id.idx * n, PS, V_LZ_BLIND + id.idx};
       case PK_LPIN: return {lpin_polys + (size_t)id.idx * n, PS, V_LPIN_BLIND + id.idx};
       case PK_LPTAB: return {lptab_polys + (size_t)id.idx * n, PS, V_LPTAB_BLIND + id.idx};
-      case PK_FIXED: return {C.fixed_polys + (size_t)id.idx * n, 0, V_ONE};
-      case PK_SIG: return {C.sig_polys + (size_t)id.idx * n, 0, V_ONE};
+      case PK_FIXED: return {C.fixed_polys.get() + (size_t)id.idx * n, 0, V_ONE};
+      case PK_SIG: return {C.sig_polys.get() + (size_t)id.idx * n, 0, V_ONE};
       case PK_H: return {h_poly.get(), nn, V_H_BLIND};
       default: return {random_poly.get(), nn, V_RANDOM_BLIND};
     }
@@ -755,7 +742,7 @@ tb_status tb_pk_commitments(tb_ctx* ctx, const tb_pk* pk, uint8_t* fixed_commitm
     DevBuf<Aff<Fq>> pts(c, cnt);
     std::vector<Fp> h(cnt, Fp::one());
     ones.upload(h.data(), cnt);
-    C->srs->commit(c, true, which ? C->sig_vals : C->fixed_vals, (long long)C->n, cnt, ones.get(), pts.get());
+    C->srs->commit(c, true, which ? C->sig_vals.get() : C->fixed_vals.get(), (long long)C->n, cnt, ones.get(), pts.get());
     fe_from_mont<Fq>(c, reinterpret_cast<Fq*>(pts.get()), 2 * (size_t)cnt);
     pts.download(which ? sigma_commitments : fixed_commitments, cnt);
     c->sync();

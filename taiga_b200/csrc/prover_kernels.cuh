@@ -19,7 +19,7 @@ inline QInstr q_make(int op, int dst, int ak, uint32_t a, int bk, uint32_t b) { 
 
 struct QProgram {           // compiled once per circuit (host), resident on the device
   std::vector<QInstr> host; int nregs = 0;
-  QInstr* dev = nullptr; int ninstr = 0;
+  DevMem<QInstr> dev; int ninstr = 0;
   int last = -1;            // index of the last constraint the program folds: its result is sum_j y^(last - j) e_j over its constraints
 };
 // Flattens the expression DAG reachable from `roots` into a register-allocated instruction list.

@@ -152,12 +152,7 @@ struct Compiler {
 void finish_program(Compiler& c, QProgram* out) {
   out->host = c.code; out->nregs = c.max_regs < 1 ? 1 : c.max_regs; out->ninstr = (int)c.code.size();
   TB_REQUIRE(out->nregs <= 48, "constraint expressions need too many live temporaries");
-  if (out->dev) cudaFree(out->dev);
-  out->dev = nullptr;
-  if (out->ninstr) {
-    TB_CUDA(cudaMalloc(&out->dev, out->ninstr * sizeof(QInstr)));
-    TB_CUDA(cudaMemcpy(out->dev, out->host.data(), out->ninstr * sizeof(QInstr), cudaMemcpyHostToDevice));
-  }
+  out->dev = out->ninstr ? DevMem<QInstr>(out->host.data(), out->ninstr) : DevMem<QInstr>();
 }
 }  // namespace
 
@@ -310,7 +305,7 @@ static void q_launch(Ctx* c, const QPartList& pl, int nregs, const QData& d, int
 }
 void q_run(Ctx* c, const QProgram& prog, const QData& d, int B) {
   QPartList pl; memset(&pl, 0, sizeof(pl));
-  pl.prog[0] = prog.dev; pl.ninstr[0] = prog.ninstr; pl.nparts = 1; pl.part_stride = 0;
+  pl.prog[0] = prog.dev.get(); pl.ninstr[0] = prog.ninstr; pl.nparts = 1; pl.part_stride = 0;
   c->work[PC_QUOT_GATES] += program_muls(prog) * (double)d.n * B;
   q_launch(c, pl, prog.nregs, d, B);
 }
@@ -319,7 +314,7 @@ void q_run_parts(Ctx* c, const std::vector<QProgram>& progs, QData d, long long 
   int nregs = 1;
   pl.nparts = (int)progs.size(); pl.part_stride = part_stride;
   for (int p = 0; p < pl.nparts; ++p) c->work[PC_QUOT_GATES] += program_muls(progs[p]) * (double)d.n * B;
-  for (int p = 0; p < pl.nparts; ++p) { pl.prog[p] = progs[p].dev; pl.ninstr[p] = progs[p].ninstr; nregs = nregs > progs[p].nregs ? nregs : progs[p].nregs; }
+  for (int p = 0; p < pl.nparts; ++p) { pl.prog[p] = progs[p].dev.get(); pl.ninstr[p] = progs[p].ninstr; nregs = nregs > progs[p].nregs ? nregs : progs[p].nregs; }
   q_launch(c, pl, nregs, d, B);
 }
 

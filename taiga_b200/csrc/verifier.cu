@@ -178,7 +178,7 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
       if (!cnt) continue;
       DevBuf<Fp> ones(ctx, cnt); DevBuf<Aff<Fq>> pts(ctx, cnt);
       std::vector<Fp> h(cnt, Fp::one()); ones.upload(h.data(), cnt);
-      srs.commit(ctx, true, which ? C.sig_vals : C.fixed_vals, (long long)n, cnt, ones.get(), pts.get());
+      srs.commit(ctx, true, which ? C.sig_vals.get() : C.fixed_vals.get(), (long long)n, cnt, ones.get(), pts.get());
       pts.download(dst.data(), cnt); ctx->sync();
     }
   }
