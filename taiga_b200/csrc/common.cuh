@@ -179,25 +179,6 @@ template <class F> inline FieldTables<F>& field_tables(Ctx* c);
 template <> inline FieldTables<Fp>& field_tables<Fp>(Ctx* c) { return c->tw_fp; }
 template <> inline FieldTables<Fq>& field_tables<Fq>(Ctx* c) { return c->tw_fq; }
 
-// 2^32-th roots of unity (pasta_curves ROOT_OF_UNITY; SURVEY B.1), canonical 32-bit LE limbs
-template <class F> TB_HD F root_of_unity_2_32();
-template <> TB_HD Fp root_of_unity_2_32<Fp>() {
-  Fp r; const uint32_t v[8] = {0xd87ea32fu, 0xbdad6fabu, 0xb7bb7584u, 0xea322bf2u, 0x0561f81au, 0x36212083u, 0xac30ebdau, 0x2bce74deu};
-  for (int i = 0; i < 8; ++i) r.l[i] = v[i]; return r.to_mont();
-}
-template <> TB_HD Fq root_of_unity_2_32<Fq>() {
-  Fq r; const uint32_t v[8] = {0x02b6d05fu, 0xa70e2c11u, 0xc106f049u, 0x9bb97ea3u, 0x492ae26eu, 0x9e5c4dfdu, 0x746d3f58u, 0x2de6a9b8u};
-  for (int i = 0; i < 8; ++i) r.l[i] = v[i]; return r.to_mont();
-}
-template <class F> TB_HD F zeta_const();  // pasta_curves ZETA (cube root of unity; halo2 coset shift)
-template <> TB_HD Fp zeta_const<Fp>() {
-  Fp r; const uint32_t v[8] = {0xfdfe4ab9u, 0x1dad5ebdu, 0x37ad3149u, 0x1d1f8bd2u, 0x57aab1b0u, 0x2caad5dcu, 0x4acdba71u, 0x12ccca83u};
-  for (int i = 0; i < 8; ++i) r.l[i] = v[i]; return r.to_mont();
-}
-template <> TB_HD Fq zeta_const<Fq>() {
-  Fq r; const uint32_t v[8] = {0x50aa0e4fu, 0x2aa9d2e0u, 0x47c033afu, 0x0fed467du, 0x1cf70f5au, 0x511db4d8u, 0x283e528eu, 0x06819a58u};
-  for (int i = 0; i < 8; ++i) r.l[i] = v[i]; return r.to_mont();
-}
 template <class F> inline F omega_k(int k) { F w = root_of_unity_2_32<F>(); for (int i = k; i < 32; ++i) w = w.sqr(); return w; }
 template <class F> inline F delta_const() { return F::from_u32(5).pow_u64(1ull << 32); }  // pasta DELTA = 5^(2^32)
 

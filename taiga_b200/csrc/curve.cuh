@@ -14,6 +14,8 @@ struct alignas(16) Aff {
   TB_HD bool is_inf() const { return x.is_zero() && y.is_zero(); }
   static TB_HD Aff inf() { Aff a; a.x = F::zero(); a.y = F::zero(); return a; }
   TB_HD Aff neg() const { Aff a; a.x = x; a.y = y.neg(); return a; }
+  TB_HD Aff to_mont() const { Aff a; a.x = x.to_mont(); a.y = y.to_mont(); return a; }
+  TB_HD Aff from_mont() const { Aff a; a.x = x.from_mont(); a.y = y.from_mont(); return a; }
 };
 
 template <class F>

@@ -7,14 +7,13 @@
 #include "common.cuh"
 #include "kernels.cuh"
 #include "srs.cuh"
+#include "transcript.cuh"
 
 namespace tb {
 
 // ---------------------------------------------------------------- transcript.cu
 enum { TR_ERR_INFINITY = 1, TR_ERR_OVERFLOW = 2 };
-struct alignas(8) TrState {
-  uint64_t h[8]; uint64_t t; uint32_t buflen, proof_len, error, pad; uint8_t buf[128];
-};
+struct TrState { Transcript tr; uint32_t proof_len, error; };
 struct Transcripts {
   Ctx* ctx = nullptr; int B = 0; uint32_t cap = 0;
   DevBuf<TrState> states; DevBuf<uint8_t> proofs;

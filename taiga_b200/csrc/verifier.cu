@@ -12,117 +12,25 @@
 #include <cstdlib>
 #include "capi_internal.cuh"
 #include "circuit.cuh"
+#include "transcript.cuh"
 
 namespace tb {
 
-// ---------------------------------------------------------------- host BLAKE2b (transcript replay)
-struct HostBlake2b {
-  uint64_t h[8], t = 0; uint8_t buf[128]; size_t buflen = 0;
-  static uint64_t rotr(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
-  explicit HostBlake2b(const char* personal16) {
-    static const uint64_t iv[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL, 0xa54ff53a5f1d36f1ULL,
-                                   0x510e527fade682d1ULL, 0x9b05688c2b3e6c1fULL, 0x1f83d9abfb41bd6bULL, 0x5be0cd19137e2179ULL};
-    memcpy(h, iv, 64); h[0] ^= 0x01010040ULL;
-    uint64_t p[2]; memcpy(p, personal16, 16); h[6] ^= p[0]; h[7] ^= p[1];
-  }
-  void compress(const uint8_t* block, bool last) {
-    static const uint64_t iv[8] = {0x6a09e667f3bcc908ULL, 0xbb67ae8584caa73bULL, 0x3c6ef372fe94f82bULL, 0xa54ff53a5f1d36f1ULL,
-                                   0x510e527fade682d1ULL, 0x9b05688c2b3e6c1fULL, 0x1f83d9abfb41bd6bULL, 0x5be0cd19137e2179ULL};
-    static const uint8_t S[12][16] = {
-        {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15}, {14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3},
-        {11, 8, 12, 0, 5, 2, 15, 13, 10, 14, 3, 6, 7, 1, 9, 4}, {7, 9, 3, 1, 13, 12, 11, 14, 2, 6, 5, 10, 4, 0, 15, 8},
-        {9, 0, 5, 7, 2, 4, 10, 15, 14, 1, 11, 12, 6, 8, 3, 13}, {2, 12, 6, 10, 0, 11, 8, 3, 4, 13, 7, 5, 15, 14, 1, 9},
-        {12, 5, 1, 15, 14, 13, 4, 10, 0, 7, 6, 3, 9, 2, 8, 11}, {13, 11, 7, 14, 12, 1, 3, 9, 5, 0, 15, 4, 8, 6, 2, 10},
-        {6, 15, 14, 9, 11, 3, 0, 8, 12, 2, 13, 7, 1, 4, 10, 5}, {10, 2, 8, 4, 7, 6, 1, 5, 15, 11, 9, 14, 3, 12, 13, 0},
-        {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15}, {14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3}};
-    uint64_t m[16], v[16];
-    memcpy(m, block, 128);
-    for (int i = 0; i < 8; ++i) { v[i] = h[i]; v[i + 8] = iv[i]; }
-    v[12] ^= t; if (last) v[14] = ~v[14];
-    auto G = [&](int a, int b, int c, int d, uint64_t x, uint64_t y) {
-      v[a] = v[a] + v[b] + x; v[d] = rotr(v[d] ^ v[a], 32); v[c] = v[c] + v[d]; v[b] = rotr(v[b] ^ v[c], 24);
-      v[a] = v[a] + v[b] + y; v[d] = rotr(v[d] ^ v[a], 16); v[c] = v[c] + v[d]; v[b] = rotr(v[b] ^ v[c], 63);
-    };
-    for (int r = 0; r < 12; ++r) {
-      const uint8_t* s = S[r];
-      G(0, 4, 8, 12, m[s[0]], m[s[1]]); G(1, 5, 9, 13, m[s[2]], m[s[3]]); G(2, 6, 10, 14, m[s[4]], m[s[5]]); G(3, 7, 11, 15, m[s[6]], m[s[7]]);
-      G(0, 5, 10, 15, m[s[8]], m[s[9]]); G(1, 6, 11, 12, m[s[10]], m[s[11]]); G(2, 7, 8, 13, m[s[12]], m[s[13]]); G(3, 4, 9, 14, m[s[14]], m[s[15]]);
-    }
-    for (int i = 0; i < 8; ++i) h[i] ^= v[i] ^ v[i + 8];
-  }
-  void update(const void* data, size_t len) {
-    const uint8_t* p = (const uint8_t*)data;
-    while (len) {
-      if (buflen == 128) { t += 128; compress(buf, false); buflen = 0; }
-      size_t take = std::min(len, (size_t)128 - buflen);
-      memcpy(buf + buflen, p, take); buflen += take; p += take; len -= take;
-    }
-  }
-  void digest(uint8_t* out) const {
-    HostBlake2b c = *this;
-    c.t += c.buflen; memset(c.buf + c.buflen, 0, 128 - c.buflen); c.compress(c.buf, true);
-    memcpy(out, c.h, 64);
-  }
-};
-
-template <class F> static bool canonical(const uint8_t* b, F& out) {  // 32 LE bytes < modulus -> Montgomery
-  F raw; memcpy(raw.l, b, 32);
-  F m; for (int i = 0; i < 8; ++i) m.l[i] = F::modulus_limb(i);
-  if (F::cmp_raw(raw, m) >= 0) return false;
-  out = raw.to_mont(); return true;
-}
-static Fp wide_reduce(const uint8_t* d64) {  // Challenge255: 64 LE bytes mod p
-  Fp lo, hi; memcpy(lo.l, d64, 32); memcpy(hi.l, d64 + 32, 32);
-  Fp r2 = Fp::r2();
-  return r2 * lo + r2 * (r2 * hi);
-}
-// Tonelli-Shanks in Fq (2-adicity 32)
-static bool fq_sqrt(const Fq& a, Fq& out) {
-  if (a.is_zero()) { out = a; return true; }
-  uint32_t q[8]; for (int i = 0; i < 8; ++i) q[i] = Fq::modulus_limb(i);
-  q[0] -= 1;                                    // m - 1 = 2^32 * odd
-  uint32_t odd[8]; for (int i = 0; i < 7; ++i) odd[i] = q[i + 1]; odd[7] = 0;
-  uint32_t h[8];                                // (odd + 1) / 2
-  { uint64_t c = 1; for (int i = 0; i < 8; ++i) { c += odd[i]; h[i] = (uint32_t)c; c >>= 32; }
-    for (int i = 0; i < 8; ++i) h[i] = (h[i] >> 1) | (i < 7 ? (h[i + 1] << 31) : 0); }
-  Fq c = root_of_unity_2_32<Fq>(), t = a.pow(odd, 8), r = a.pow(h, 8);
-  int m = 32;
-  Fq one = Fq::one();
-  while (t != one) {
-    int i = 0; Fq t2 = t;
-    while (t2 != one) { t2 = t2.sqr(); if (++i == m) return false; }
-    Fq b = c; for (int j = 0; j < m - i - 1; ++j) b = b.sqr();
-    m = i; c = b.sqr(); t = t * c; r = r * b;
-  }
-  out = r; return true;
-}
-static bool decompress(const uint8_t* b, Aff<Fq>& out) {  // pasta encoding: x LE, bit 255 = parity of y; identity = zeros
-  uint8_t t[32]; memcpy(t, b, 32);
-  int sign = t[31] >> 7; t[31] &= 0x7f;
-  bool allz = true; for (int i = 0; i < 32; ++i) allz &= (t[i] == 0);
-  if (allz && !sign) { out = Aff<Fq>::inf(); return true; }
-  Fq x; if (!canonical<Fq>(t, x)) return false;
-  Fq y; if (!fq_sqrt(x.sqr() * x + Fq::from_u32(5), y)) return false;
-  if ((int)(y.from_mont().l[0] & 1) != sign) y = y.neg();
-  out.x = x; out.y = y; return true;
-}
-
-struct VTranscript {
-  HostBlake2b st; const uint8_t* rd; size_t len, pos = 0; bool bad = false;
-  VTranscript(const uint8_t* p, size_t n) : st("Halo2-Transcript"), rd(p), len(n) {}
-  void common_point(const Aff<Fq>& p) {
-    if (p.is_inf()) { bad = true; return; }
-    uint8_t b[65]; b[0] = 1; Fq x = p.x.from_mont(), y = p.y.from_mont(); memcpy(b + 1, x.l, 32); memcpy(b + 33, y.l, 32); st.update(b, 65);
-  }
-  void common_scalar(const Fp& s) { uint8_t b[33]; b[0] = 2; Fp c = s.from_mont(); memcpy(b + 1, c.l, 32); st.update(b, 33); }
-  Fp squeeze() { uint8_t z = 0; st.update(&z, 1); uint8_t d[64]; st.digest(d); return wide_reduce(d); }
+// the transcript replayed over the bytes of one proof; `bad` once a read failed or the identity was absorbed
+struct VTranscript : Transcript {
+  const uint8_t* rd; size_t len, pos = 0; bool bad = false;
+  VTranscript(const uint8_t* p, size_t n, const Fp& vk_repr) : rd(p), len(n) { start(vk_repr); }
+  void common_point(const Aff<Fq>& p) { if (!absorb_point(p.from_mont())) bad = true; }
   bool read_point(Aff<Fq>& p) {
-    if (pos + 32 > len || !decompress(rd + pos, p)) { bad = true; return false; }
-    pos += 32; common_point(p); return !bad;
+    Aff<Fq> c;
+    if (pos + 32 > len || !decompress_point(rd + pos, c)) { bad = true; return false; }
+    pos += 32;
+    if (!absorb_point(c)) bad = true;
+    p = c.to_mont(); return !bad;
   }
   bool read_scalar(Fp& s) {
     if (pos + 32 > len || !canonical<Fp>(rd + pos, s)) { bad = true; return false; }
-    pos += 32; common_scalar(s); return true;
+    pos += 32; absorb_scalar(s.from_mont()); return true;
   }
 };
 
@@ -212,8 +120,7 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
   Fp omega = C.omega, omega_inv = C.omega.inv(), n_inv = Fp::from_u32((uint32_t)n).inv();
   auto rot_pow = [&](int rot) { Fp r = one; const Fp& w = rot >= 0 ? omega : omega_inv; for (int i = 0; i < std::abs(rot); ++i) r = r * w; return r; };
   for (int p = 0; p < K; ++p) {
-    VTranscript tr(proofs + (size_t)p * proof_stride, proof_len);
-    { Fp repr = C.vk_repr.to_mont(); tr.common_scalar(repr); }
+    VTranscript tr(proofs + (size_t)p * proof_stride, proof_len, C.vk_repr);
     bool ok = true;
     const uint8_t* ib = instance + 32 * inst_total * p;
     for (size_t i = 0; i < inst_total && ok; ++i) { Fp t; ok = canonical<Fp>(ib + 32 * i, t); }

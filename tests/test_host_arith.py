@@ -1,6 +1,8 @@
-"""CPU: the product's own field/curve source (taiga_b200/csrc/field.cuh, curve.cuh - the code the kernels compile)
-instantiated for the host and checked against the Python big-int oracle."""
+"""CPU: the product's own field/curve and transcript source (taiga_b200/csrc/field.cuh, curve.cuh, transcript.cuh - the
+code the kernels and the verifier compile) instantiated for the host and checked against the Python big-int oracle, hashlib
+and the independent Python verifier."""
 import ctypes
+import hashlib
 import os
 import random
 import subprocess
@@ -64,3 +66,136 @@ def test_curve(shim):
         assert po(c, 3, A, B) == cv.add(cv.mul(2, A), cv.mul(3, B)) and po(c, 3, A, A) == cv.mul(5, A)
         for k in [0, 1, 2, 15, 16, cv.fs - 1, rnd.randrange(cv.fs)]:
             assert po(c, 1, A, _b32(k)) == cv.mul(k, A)
+
+
+# ---------------------------------------------------------------- transcript.cuh: BLAKE2b, transcript, PRF, encodings
+def _buf(b):
+    return (ctypes.c_uint8 * max(1, len(b))).from_buffer_copy(bytes(b) or b"\0")
+
+
+def _out(shim_fn, *args, n=32):
+    out = (ctypes.c_uint8 * n)()
+    shim_fn(*args, out)
+    return bytes(out)
+
+
+def _points(rnd, count):
+    """count consecutive multiples of the Vesta generator from a random start, and their negations"""
+    pts = [o.VESTA.mul(rnd.randrange(1, o.P), o.VESTA_GEN)]
+    while len(pts) < count:
+        pts.append(o.VESTA.add(pts[-1], o.VESTA_GEN))
+    return pts + [o.VESTA.neg(p) for p in pts]
+
+
+def test_blake2b_matches_hashlib(shim):
+    rnd = random.Random(7)
+    for person in (b"Halo2-Transcript", b"TaigaB200-Blind\0"):
+        for n in (0, 1, 127, 128, 129, 255, 256, 257, 1000):
+            data = bytes(rnd.randrange(256) for _ in range(n))
+            ref = hashlib.blake2b(data, digest_size=64, person=person).digest()
+            chunkings = [[n]]
+            for _ in range(4):   # random cuts, empty pieces included
+                cuts = sorted(rnd.randrange(n + 1) for _ in range(rnd.randrange(1, 6)))
+                chunkings.append([b - a for a, b in zip([0] + cuts, cuts + [n])])
+            for ch in chunkings:
+                got = _out(shim.hs_blake2b, person, _buf(data), (ctypes.c_int * len(ch))(*ch), len(ch), n=64)
+                assert got == ref, (person, n, ch)
+
+
+def test_transcript_matches_oracle(shim):
+    """Random interleavings of points, scalars and squeezes; every script squeezes once with exactly a multiple of 128
+    bytes absorbed, where the last full block must stay buffered and be compressed as the final one."""
+    rnd = random.Random(8)
+    pts = _points(rnd, 16)
+    boundary_squeezes = 0
+    for _ in range(12):
+        vk = rnd.randrange(o.P)
+        ref = o.Transcript()
+        ref.common_scalar(vk)
+        ops, data, want = [], b"", []
+        absorbed = 33
+        pad_at = rnd.randrange(40)
+        for i in range(40):
+            kinds = [rnd.choice("PSZ")]
+            if i == pad_at:   # a squeeze absorbs one byte: squeeze up to the next block boundary
+                kinds = ["Z"] * (-absorbed % 128 or 128)
+            for kind in kinds:
+                if kind == "P":
+                    p = rnd.choice(pts)
+                    ref.common_point(p)
+                    data += o.to_bytes(p[0]) + o.to_bytes(p[1])
+                    absorbed += 65
+                elif kind == "S":
+                    s = rnd.randrange(o.P)
+                    ref.common_scalar(s)
+                    data += o.to_bytes(s)
+                    absorbed += 33
+                else:
+                    want.append(ref.squeeze())
+                    absorbed += 1
+                    boundary_squeezes += absorbed % 128 == 0
+                ops.append(kind)
+        out = (ctypes.c_uint8 * (32 * len(want)))()
+        assert shim.hs_transcript(_b32(vk), "".join(ops).encode(), len(ops), _buf(data), out) == -1
+        assert [int.from_bytes(bytes(out)[32 * i:32 * i + 32], "little") for i in range(len(want))] == want
+    assert boundary_squeezes >= 12
+    # the identity is refused, as halo2's common_point refuses it
+    with pytest.raises(ValueError):
+        o.Transcript().common_point(None)
+    assert shim.hs_transcript(_b32(0), b"SP", 2, _buf(bytes(96)), (ctypes.c_uint8 * 32)()) == 1
+
+
+def test_prf_matches_hashlib(shim):
+    seed = bytes(range(32))
+    for proof, tag, idx in ((0, 1, 0), (5, 11, 32767), (1 << 20, 18, 14), (2 ** 32 - 1, 18, 2 ** 15 - 1)):
+        m = seed + proof.to_bytes(4, "little") + tag.to_bytes(4, "little") + idx.to_bytes(4, "little") + bytes(4)
+        ref = int.from_bytes(hashlib.blake2b(m, digest_size=64, person=b"TaigaB200-Blind\0").digest(), "little") % o.P
+        assert int.from_bytes(_out(shim.hs_prf, _buf(seed), proof, tag, idx), "little") == ref
+
+
+def test_point_and_scalar_encodings(shim):
+    from oracle import verifier_py as vp
+    from taiga_b200 import circuits_mini as cm
+    import soundness_cases as sc
+
+    def dec(enc):
+        xy = (ctypes.c_uint8 * 64)()
+        if not shim.hs_decompress(_buf(enc), xy):
+            return "reject"
+        r = bytes(xy)
+        x, y = int.from_bytes(r[:32], "little"), int.from_bytes(r[32:], "little")
+        return None if x == 0 and y == 0 else (x, y)
+
+    def ref_dec(enc):
+        try:
+            p = vp.decompress(enc)
+        except vp.Reject:
+            return "reject"
+        return None if p[2] == 0 else vp._to_affine(p)
+
+    for p in _points(random.Random(9), 32) + [None]:
+        assert _out(shim.hs_compress, _b64(p)) == o.VESTA.compress(p)
+    kd, _ = cm.standard_plonk(k=6, wide=False, n_lookups=2)
+    proof = open(os.path.join(ROOT, "tests", "golden", "proof_k6_plonk.bin"), "rb").read()
+    slots = sc.slots(kd)
+    assert len(proof) == slots[-1][2] + 32
+    n_points = 0
+    for name, e, off, kind in slots:
+        v = int.from_bytes(proof[off:off + 32], "little")
+        if kind == "point":
+            n_points += 1
+            x, sign = v & ((1 << 255) - 1), v >> 255
+            for enc in (v, v ^ (1 << 255)):
+                b = enc.to_bytes(32, "little")
+                assert dec(b) == ref_dec(b) != "reject", (name, e)
+            bad = [1 << 255, sc.OFF_CURVE_X | sign << 255, (1 << 256) - 1] + ([(x + vp.Q) | sign << 255] if x + vp.Q < 1 << 255 else [])
+            for enc in bad:
+                b = enc.to_bytes(32, "little")
+                assert dec(b) == ref_dec(b) == "reject", (name, e, hex(enc))
+        else:
+            for enc, ok in ((v, True), (v + o.P, False), ((1 << 256) - 1, False)):
+                out = (ctypes.c_uint8 * 32)()
+                assert shim.hs_scalar(_buf(enc.to_bytes(32, "little")), out) == ok, (name, e, hex(enc))
+                assert not ok or int.from_bytes(bytes(out), "little") == v
+    assert n_points > 20
+    assert dec(bytes(32)) is None and ref_dec(bytes(32)) is None
