@@ -39,7 +39,7 @@ struct Circuit {
   std::vector<QProgram> gate_parts[2], gate_parts_lo[2];
   bool split = false; uint32_t num_constraints = 0, t_pl = 0;   // t_pl: permutation + lookup terms folded after the gates
   std::vector<Fp> t_inv; Fp delta, zeta, omega, r_inv;
-  Fp delta_c0[16];
+  Fp delta_c0[PERM_MAX_SETS];
   // evaluation / multiopen structure (host)
   std::vector<QueryRef> evals;            // transcript order of the evaluation section
   std::vector<QueryRef> queries;          // multiopen query order

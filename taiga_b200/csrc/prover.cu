@@ -34,7 +34,7 @@ static void to_cosets(Ctx* ctx, const Circuit& C, const Fp* polys, Fp* cosets, F
 
 static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, const uint8_t* fixed, const uint8_t* sigma) {
   TB_REQUIRE(cs->k == srs->k, "circuit k must match the SRS");
-  TB_REQUIRE(cs->cs_degree >= 3 && cs->num_perm_columns <= 16 * (cs->cs_degree - 2), "unsupported constraint system shape");
+  TB_REQUIRE(cs->cs_degree >= 3 && cs->num_perm_columns <= PERM_MAX_SETS * (cs->cs_degree - 2), "unsupported constraint system shape");
   std::unique_ptr<Circuit> Cp(new Circuit());
   Circuit& C = *Cp;
   C.srs = srs;
@@ -91,7 +91,7 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
 
   C.delta = delta_const<Fp>(); C.zeta = zeta_const<Fp>(); C.omega = omega_k<Fp>((int)C.k);
   C.r_inv = Fp::from_u32((uint32_t)C.R).inv();
-  for (uint32_t s = 0; s < 16; ++s) C.delta_c0[s] = C.delta.pow_u64((uint64_t)s * C.chunk);
+  for (int s = 0; s < PERM_MAX_SETS; ++s) C.delta_c0[s] = C.delta.pow_u64((uint64_t)s * C.chunk);
   Fp w_ext = omega_k<Fp>(C.ext_k);
   { Fp zn = C.zeta.pow_u64(C.n), step = w_ext.pow_u64(C.n), cur = zn;
     for (int k1 = 0; k1 < C.R; ++k1) { C.t_inv.push_back((cur - Fp::one()).inv()); cur = cur * step; }
@@ -140,7 +140,7 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   // expression programs (descriptor rebuilt from the deep copy so pointers stay valid)
   { tb_cs_desc d = *cs;
     C.num_constraints = cs->num_constraints;
-    C.t_pl = (C.nsets ? 2 + (C.nsets - 1) + C.nsets : 0) + 5 * C.L;
+    C.t_pl = perm_lookup_terms(C.nsets, C.L);
     // Degree split: a constraint of degree <= R / 2 is a polynomial of fewer than (R / 2) * n coefficients, so the sum of all such
     // constraints is fixed by its values on every second sub-coset; only the high-degree constraints (and the permutation /
     // lookup terms) need all R sub-cosets.  Worth it when the low class carries a good part of the arithmetic.

@@ -1,5 +1,6 @@
 // Declarations for lookup.cu and quotient.cu (kernel drivers used by prover.cu).
 #pragma once
+#include "argument.cuh"
 #include "prover.cuh"
 
 namespace tb {
@@ -62,7 +63,7 @@ struct QFinish {
   const int2* perm_cols; int P; int chunk; int nsets; int L; int bf;
   const Fp* chal; long long chal_stride; int y_slot, beta_slot, gamma_slot;
   Fp delta; Fp zeta; Fp t_inv;                       // DELTA, ZETA, 1/((zeta w^k1)^n - 1)
-  Fp delta_c0[16];                                   // DELTA^(s*chunk) per permutation set
+  Fp delta_c0[PERM_MAX_SETS];                        // DELTA^(s*chunk) per permutation set
   TwiddleTables<Fp> tw;                              // forward tables
   int ext_k; int k;
   Fp* out; long long out_pstride;                    // H[b][k1][row]  (out + b*out_pstride + k1*n + row)
@@ -89,7 +90,7 @@ struct PermFrac {
   const int2* perm_cols; int P; int chunk; int nsets;
   const Fp* chal; long long chal_stride; int beta_slot, gamma_slot;
   Fp delta, omega;
-  Fp delta_c0[16];
+  Fp delta_c0[PERM_MAX_SETS];
   TwiddleTables<Fp> tw;
   Fp* num; Fp* den; long long pstride;   // [B][nsets][n]
   int n; int k;

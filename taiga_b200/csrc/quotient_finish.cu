@@ -7,6 +7,23 @@
 
 namespace tb {
 
+// One row of one proof on one sub-coset of the extended domain, or of the Lagrange values (R = 1, k1 = 0): the view
+// through which argument.cuh reads the permutation columns, the sigma polynomials and (q_finish only) the permutation
+// grand products.  Fixed and sigma columns are [col][R][n], the other columns [col][n]; rows wrap around.
+struct RowView {
+  const Fp* adv; const Fp* inst; const Fp* fix; const Fp* sig; const int2* cols; const Fp* pz;
+  int R, k1, n, row, last_rot;
+  __device__ __forceinline__ Fp perm_col(int c) const {
+    const int2 col = cols[c];
+    return col.x == TB_COL_ADVICE ? ldg_fe(adv + (size_t)col.y * n + row)
+         : col.x == TB_COL_FIXED ? ldg_fe(fix + ((size_t)col.y * R + k1) * n + row) : ldg_fe(inst + (size_t)col.y * n + row);
+  }
+  __device__ __forceinline__ Fp sigma(int c) const { return ldg_fe(sig + ((size_t)c * R + k1) * n + row); }
+  __device__ __forceinline__ Fp z(int s) const { return ldg_fe(pz + (size_t)s * n + row); }
+  __device__ __forceinline__ Fp z_next(int s) const { return ldg_fe(pz + (size_t)s * n + ((row + 1) & (n - 1))); }
+  __device__ __forceinline__ Fp z_last(int s) const { return ldg_fe(pz + (size_t)s * n + ((row + last_rot + n) & (n - 1))); }
+};
+
 // ---------------------------------------------------------------- permutation + lookup terms, vanishing division
 __global__ void __launch_bounds__(128) q_finish_kernel(QFinish f) {
   const int row = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
@@ -14,48 +31,23 @@ __global__ void __launch_bounds__(128) q_finish_kernel(QFinish f) {
   const int n = f.n, nm = n - 1;
   const Fp* chal = f.chal + (long long)b * f.chal_stride;
   const Fp y = chal[f.y_slot], beta = chal[f.beta_slot], gamma = chal[f.gamma_slot];
-  const Fp one = Fp::one();
   const size_t crow = (size_t)f.k1 * n + row;
   Fp acc = Fp::zero();   // gate programs: sum_p y^(J - 1 - last_p) S_p
   for (int p = 0; p < f.nparts; ++p) acc = acc + chal[f.ytab_slot + f.gexp[p]] * ldg_fe(f.gate + (size_t)p * f.gate_part_stride + (size_t)b * n + row);
-  const Fp l0 = ldg_fe(f.l0 + crow), ll = ldg_fe(f.l_last + crow);
-  const Fp active = one - (ll + ldg_fe(f.l_blind + crow));
-  const Fp* adv = f.adv + (long long)b * f.adv_pstride;
-  const Fp* inst = f.inst + (long long)b * f.inst_pstride;
-  if (f.nsets) {
-    const Fp* pz = f.pz + (long long)b * f.pz_pstride;
-    const int last_rot = -(f.bf + 1);
-    acc = acc * y + l0 * (one - ldg_fe(pz + row));
-    { Fp zl = ldg_fe(pz + (size_t)(f.nsets - 1) * n + row); acc = acc * y + ll * (zl * zl - zl); }
-    for (int s = 1; s < f.nsets; ++s)
-      acc = acc * y + l0 * (ldg_fe(pz + (size_t)s * n + row) - ldg_fe(pz + (size_t)(s - 1) * n + ((row + last_rot + n) & nm)));
-    // X on this sub-coset: zeta * w_ext^(k1 + R*row)
-    Fp xcur = f.zeta * tw_pow(f.tw, (uint32_t)(f.k1 + f.R * row) << (TW_LOG - f.ext_k));
-    for (int s = 0; s < f.nsets; ++s) {
-      int c0 = s * f.chunk, c1 = c0 + f.chunk < f.P ? c0 + f.chunk : f.P;
-      Fp left = ldg_fe(pz + (size_t)s * n + ((row + 1) & nm)), right = ldg_fe(pz + (size_t)s * n + row);
-      Fp cd = beta * f.delta_c0[s] * xcur;
-      for (int cidx = c0; cidx < c1; ++cidx) {
-        int2 col = f.perm_cols[cidx];
-        Fp val = col.x == TB_COL_ADVICE ? ldg_fe(adv + (size_t)col.y * n + row)
-               : col.x == TB_COL_FIXED ? ldg_fe(f.fix + ((size_t)col.y * f.R + f.k1) * n + row) : ldg_fe(inst + (size_t)col.y * n + row);
-        left = left * (val + beta * ldg_fe(f.sig + ((size_t)cidx * f.R + f.k1) * n + row) + gamma);
-        right = right * (val + cd + gamma);
-        cd = cd * f.delta;
-      }
-      acc = acc * y + (left - right) * active;
-    }
+  const Fp ll = ldg_fe(f.l_last + crow);
+  const ArgPoint at = {y, beta, gamma, ldg_fe(f.l0 + crow), ll, Fp::one() - (ll + ldg_fe(f.l_blind + crow))};
+  if (f.nsets) {   // without a permutation, X and its twiddle loads are not needed
+    const RowView v = {f.adv + (long long)b * f.adv_pstride, f.inst + (long long)b * f.inst_pstride, f.fix, f.sig, f.perm_cols, f.pz + (long long)b * f.pz_pstride,
+                       f.R, f.k1, n, row, -(f.bf + 1)};
+    const Fp x = f.zeta * tw_pow(f.tw, (uint32_t)(f.k1 + f.R * row) << (TW_LOG - f.ext_k));   // zeta * w_ext^(k1 + R*row)
+    acc = perm_fold(acc, v, at, f.nsets, f.chunk, f.P, f.delta, f.delta_c0, x);
   }
   for (int l = 0; l < f.L; ++l) {
     size_t o = (size_t)b * f.lk_pstride + (size_t)l * n, oc = (size_t)b * f.lkc_pstride + (size_t)l * n;
     Fp z = ldg_fe(f.lz + o + row), zn = ldg_fe(f.lz + o + ((row + 1) & nm));
     Fp ap = ldg_fe(f.lpin + o + row), apm = ldg_fe(f.lpin + o + ((row - 1 + n) & nm)), sp = ldg_fe(f.lptab + o + row);
     Fp a = ldg_fe(f.lkA + oc + row), t = ldg_fe(f.lkS + oc + row);
-    acc = acc * y + l0 * (one - z);
-    acc = acc * y + ll * (z * z - z);
-    acc = acc * y + (zn * (ap + beta) * (sp + gamma) - z * (a + beta) * (t + gamma)) * active;
-    acc = acc * y + l0 * (ap - sp);
-    acc = acc * y + (ap - sp) * (ap - apm) * active;
+    acc = lookup_fold(acc, at, z, zn, ap, apm, sp, a, t);
   }
   if (f.rlo) acc = acc + ldg_fe(f.rlo + (long long)b * f.rlo_pstride + row);   // low-degree numerator modulo X^n - 1 (its quotient is added in coefficient form)
   st_fe(f.out + (long long)b * f.out_pstride + crow, acc * f.t_inv);
@@ -139,19 +131,9 @@ __global__ void perm_fractions_kernel(PermFrac p) {
   const int n = p.n;
   const Fp* chal = p.chal + (long long)b * p.chal_stride;
   const Fp beta = chal[p.beta_slot], gamma = chal[p.gamma_slot];
-  const Fp* adv = p.adv + (long long)b * p.adv_pstride;
-  const Fp* inst = p.inst + (long long)b * p.inst_pstride;
-  int c0 = s * p.chunk, c1 = c0 + p.chunk < p.P ? c0 + p.chunk : p.P;
+  const RowView v = {p.adv + (long long)b * p.adv_pstride, p.inst + (long long)b * p.inst_pstride, p.fix, p.sig, p.perm_cols, nullptr, 1, 0, n, row, 0};
   Fp num = Fp::one(), den = Fp::one();
-  Fp dw = p.delta_c0[s] * tw_pow(p.tw, (uint32_t)row << (TW_LOG - p.k)) * beta;  // delta^c * omega^row * beta
-  for (int cidx = c0; cidx < c1; ++cidx) {
-    int2 col = p.perm_cols[cidx];
-    Fp val = col.x == TB_COL_ADVICE ? ldg_fe(adv + (size_t)col.y * n + row)
-           : col.x == TB_COL_FIXED ? ldg_fe(p.fix + (size_t)col.y * n + row) : ldg_fe(inst + (size_t)col.y * n + row);
-    den = den * (beta * ldg_fe(p.sig + (size_t)cidx * n + row) + gamma + val);
-    num = num * (dw + gamma + val);
-    dw = dw * p.delta;
-  }
+  perm_set_products(v, s, p.chunk, p.P, beta, gamma, p.delta, p.delta_c0[s] * tw_pow(p.tw, (uint32_t)row << (TW_LOG - p.k)) * beta, den, num);   // X = omega^row
   size_t o = (size_t)b * p.pstride + (size_t)s * n + row;
   st_fe(p.num + o, num); st_fe(p.den + o, den);
 }
@@ -194,8 +176,8 @@ __global__ void lookup_fractions_kernel(const Fp* A, const Fp* S, const Fp* Ap, 
   if (row >= n) return;
   const Fp beta = chal[(long long)b * chal_stride + beta_slot], gamma = chal[(long long)b * chal_stride + gamma_slot];
   size_t o = (size_t)b * pstride + (size_t)l * n + row;
-  st_fe(den + o, (beta + ld_fe(Ap + o)) * (gamma + ld_fe(Sp + o)));
-  st_fe(num + o, (ld_fe(A + o) + beta) * (ld_fe(S + o) + gamma));
+  st_fe(den + o, lookup_factor(ld_fe(Ap + o), ld_fe(Sp + o), beta, gamma));
+  st_fe(num + o, lookup_factor(ld_fe(A + o), ld_fe(S + o), beta, gamma));
 }
 void lookup_fractions(Ctx* c, const Fp* A, const Fp* S, const Fp* Ap, const Fp* Sp, Fp* num, Fp* den, long long pstride, int L, int n,
                       const Fp* chal, long long chal_stride, int beta_slot, int gamma_slot, int B) {

@@ -69,6 +69,16 @@ static Fp eval_expr(const Circuit& C, uint32_t root, std::vector<Fp>& memo, std:
   return r;
 }
 
+// the proof's evaluations at x, as argument.cuh reads them
+struct EvalView {
+  const Circuit& C; std::map<std::pair<PolyId, int>, Fp>& ev; int last_rot;
+  Fp perm_col(int c) const { const tb_column& col = C.perm[c]; return ev[{{col.kind == TB_COL_ADVICE ? PK_ADV : col.kind == TB_COL_FIXED ? PK_FIXED : PK_INST, (int)col.index}, 0}]; }
+  Fp sigma(int c) const { return ev[{{PK_SIG, c}, 0}]; }
+  Fp z(int s) const { return ev[{{PK_PZ, s}, 0}]; }
+  Fp z_next(int s) const { return ev[{{PK_PZ, s}, 1}]; }
+  Fp z_last(int s) const { return ev[{{PK_PZ, s}, last_rot}]; }
+};
+
 static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride,
                          size_t proof_len, uint8_t* ok_out) {
   const Srs& srs = *C.srs;
@@ -160,33 +170,13 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     std::vector<Fp> memo(C.nodes.size()); std::vector<char> done(C.nodes.size(), 0);
     Fp acc = Fp::zero();
     for (uint32_t r : C.roots) acc = acc * y + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
-    Fp active = one - (l_last + l_blind);
-    auto col_eval = [&](const tb_column& c) { return ev[{{c.kind == TB_COL_ADVICE ? PK_ADV : c.kind == TB_COL_FIXED ? PK_FIXED : PK_INST, (int)c.index}, 0}]; };
-    if (nsets) {
-      auto pz = [&](int s, int rot) { return ev[{{PK_PZ, s}, rot}]; };
-      acc = acc * y + l_0 * (one - pz(0, 0));
-      acc = acc * y + (pz(nsets - 1, 0).sqr() - pz(nsets - 1, 0)) * l_last;
-      for (int s = 1; s < nsets; ++s) acc = acc * y + (pz(s, 0) - pz(s - 1, last_rot)) * l_0;
-      for (int s = 0; s < nsets; ++s) {
-        int c0 = s * (int)C.chunk, c1 = std::min(P, c0 + (int)C.chunk);
-        Fp left = pz(s, 1), right = pz(s, 0), cd = beta * x * C.delta_c0[s];
-        for (int c = c0; c < c1; ++c) {
-          Fp e = col_eval(C.perm[c]);
-          left = left * (e + beta * ev[{{PK_SIG, c}, 0}] + gamma); right = right * (e + cd + gamma); cd = cd * C.delta;
-        }
-        acc = acc * y + (left - right) * active;
-      }
-    }
+    const ArgPoint at = {y, beta, gamma, l_0, l_last, one - (l_last + l_blind)};
+    acc = perm_fold(acc, EvalView{C, ev, last_rot}, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
     for (int l = 0; l < L; ++l) {
       Fp a = Fp::zero(), t = Fp::zero();
       for (uint32_t r : C.lk_in[l]) a = a * theta + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
       for (uint32_t r : C.lk_tab[l]) t = t * theta + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
-      Fp z = ev[{{PK_LZ, l}, 0}], zn = ev[{{PK_LZ, l}, 1}], ap = ev[{{PK_LPIN, l}, 0}], am = ev[{{PK_LPIN, l}, -1}], sp = ev[{{PK_LPTAB, l}, 0}];
-      acc = acc * y + l_0 * (one - z);
-      acc = acc * y + l_last * (z.sqr() - z);
-      acc = acc * y + (zn * (ap + beta) * (sp + gamma) - z * (a + beta) * (t + gamma)) * active;
-      acc = acc * y + l_0 * (ap - sp);
-      acc = acc * y + (ap - sp) * (ap - am) * active;
+      acc = lookup_fold(acc, at, ev[{{PK_LZ, l}, 0}], ev[{{PK_LZ, l}, 1}], ev[{{PK_LPIN, l}, 0}], ev[{{PK_LPIN, l}, -1}], ev[{{PK_LPTAB, l}, 0}], a, t);
     }
     ev[{{PK_H, 0}, 0}] = acc * (xn - one).inv();
     // ---- multiopen

@@ -1,6 +1,7 @@
-// Host instantiation of the product's __host__ __device__ field/curve arithmetic and transcript (taiga_b200/csrc/*.cuh),
-// so the same source the kernels compile can be checked on a CPU-only box against the oracle.
+// Host instantiation of the product's __host__ __device__ field/curve arithmetic, transcript and argument terms
+// (taiga_b200/csrc/*.cuh), so the same source the kernels compile can be checked on a CPU-only box against the oracle.
 #include <cstring>
+#include "../taiga_b200/csrc/argument.cuh"
 #include "../taiga_b200/csrc/transcript.cuh"
 using namespace tb;
 template <class F> static void fop(int op, const uint8_t* a, const uint8_t* b, uint8_t* o) {
@@ -48,4 +49,41 @@ void hs_compress(const uint8_t* xy, uint8_t* out) { Aff<Fq> p; memcpy(&p, xy, 64
 int hs_decompress(const uint8_t* b, uint8_t* xy) { Aff<Fq> p; if (!decompress_point(b, p)) return 0; memcpy(xy, &p, 64); return 1; }
 // a scalar of the proof; on success out = the value back from Montgomery form
 int hs_scalar(const uint8_t* b, uint8_t* out) { Fp v; if (!canonical<Fp>(b, v)) return 0; v = v.from_mont(); memcpy(out, v.l, 32); return 1; }
+}
+
+// ---------------------------------------------------------------- argument.cuh; every value canonical, 32 bytes
+static Fp fe(const uint8_t* b) { Fp v; memcpy(v.l, b, 32); return v.to_mont(); }
+static void put(const Fp& v, uint8_t* out) { Fp c = v.from_mont(); memcpy(out, c.l, 32); }
+// permutation column c is vals[kind[c]][index[c]] (kinds advice, fixed, instance); zs is [set][X, wX, w^-(bf+1) X]
+struct ShimView {
+  const int* kind; const int* index; const uint8_t* vals[3]; const uint8_t* sig; const uint8_t* zs;
+  Fp perm_col(int c) const { return fe(vals[kind[c]] + 32 * index[c]); }
+  Fp sigma(int c) const { return fe(sig + 32 * c); }
+  Fp z(int s) const { return fe(zs + 96 * s); }
+  Fp z_next(int s) const { return fe(zs + 96 * s + 32); }
+  Fp z_last(int s) const { return fe(zs + 96 * s + 64); }
+};
+extern "C" {
+// out = [prod with sigma, prod with the identity] of set s, both products started at one
+void hs_perm_set(const int* kind, const int* index, const uint8_t* adv, const uint8_t* fix, const uint8_t* inst, const uint8_t* sig, int s, int chunk, int ncols,
+                 const uint8_t* beta, const uint8_t* gamma, const uint8_t* delta, const uint8_t* cd, uint8_t* out) {
+  ShimView v = {kind, index, {adv, fix, inst}, sig, nullptr};
+  Fp with_sigma = Fp::one(), with_id = Fp::one();
+  perm_set_products(v, s, chunk, ncols, fe(beta), fe(gamma), fe(delta), fe(cd), with_sigma, with_id);
+  put(with_sigma, out); put(with_id, out + 32);
+}
+// acc after the permutation terms and L lookups' terms; pt = acc, x, y, beta, gamma, l0, l_last, active;
+// lk = [L][z, z_next, ap, ap_prev, sp, a, s]
+void hs_arg_fold(const uint8_t* pt, const uint8_t* delta, const int* kind, const int* index, const uint8_t* adv, const uint8_t* fix, const uint8_t* inst,
+                 const uint8_t* sig, const uint8_t* zs, int nsets, int chunk, int ncols, int L, const uint8_t* lk, uint8_t* out) {
+  ShimView v = {kind, index, {adv, fix, inst}, sig, zs};
+  Fp d = fe(delta), delta_c0[PERM_MAX_SETS];
+  for (int s = 0; s < PERM_MAX_SETS; ++s) delta_c0[s] = d.pow_u64((uint64_t)s * chunk);
+  const ArgPoint at = {fe(pt + 64), fe(pt + 96), fe(pt + 128), fe(pt + 160), fe(pt + 192), fe(pt + 224)};
+  Fp acc = perm_fold(fe(pt), v, at, nsets, chunk, ncols, d, delta_c0, fe(pt + 32));
+  for (int l = 0; l < L; ++l, lk += 224)
+    acc = lookup_fold(acc, at, fe(lk), fe(lk + 32), fe(lk + 64), fe(lk + 96), fe(lk + 128), fe(lk + 160), fe(lk + 192));
+  put(acc, out);
+}
+uint32_t hs_arg_terms(uint32_t nsets, uint32_t L) { return perm_lookup_terms(nsets, L); }
 }

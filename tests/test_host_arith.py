@@ -199,3 +199,101 @@ def test_point_and_scalar_encodings(shim):
                 assert not ok or int.from_bytes(bytes(out), "little") == v
     assert n_points > 20
     assert dec(bytes(32)) is None and ref_dec(bytes(32)) is None
+
+
+# ---------------------------------------------------------------- argument.cuh: permutation and lookup terms
+def _fes(vals):
+    return _buf(b"".join(o.to_bytes(v) for v in vals))
+
+
+def _ints(vals):
+    return (ctypes.c_int * max(1, len(vals)))(*vals)
+
+
+def _perm_case(rnd, chunk, ncols, per_kind=3):
+    """random permutation columns of every kind (each kind appears once there are 3 columns), values and sigmas"""
+    kinds = [c % 3 for c in range(ncols)]
+    rnd.shuffle(kinds)
+    cols = [(k, rnd.randrange(per_kind)) for k in kinds]
+    vals = [[rnd.randrange(o.P) for _ in range(per_kind)] for _ in range(3)]
+    sig = [rnd.randrange(o.P) for _ in range(ncols)]
+    return cols, vals, sig
+
+
+def _ref_arg_terms(cols, vals, sig, pz, lk, x, beta, gamma, l_0, l_last, active, chunk):
+    """oracle/verifier_py.py's permutation and lookup terms, from the same evaluations (pz[s] = z_s at x, wx, w^-(bf+1) x;
+    lk[l] = Z(x), Z(wx), A'(x), A'(w^-1 x), S'(x) and the compressed input and table)"""
+    P, DELTA, nsets = o.P, o.DELTA_P, len(pz)
+    terms = []
+    if nsets:
+        terms.append(l_0 * (1 - pz[0][0]) % P)
+        zl = pz[-1][0]
+        terms.append(l_last * (zl * zl - zl) % P)
+        for s in range(1, nsets):
+            terms.append(l_0 * (pz[s][0] - pz[s - 1][2]) % P)
+        for s in range(nsets):
+            left, right = pz[s][1], pz[s][0]
+            cur = beta * x % P * pow(DELTA, s * chunk, P) % P
+            for ci, (kind, idx) in enumerate(cols[s * chunk:(s + 1) * chunk]):
+                v = vals[kind][idx]
+                left = left * (v + beta * sig[s * chunk + ci] + gamma) % P
+                right = right * (v + cur + gamma) % P
+                cur = cur * DELTA % P
+            terms.append((left - right) * active % P)
+    for z, zn, ap, apm, sp, a_c, t_c in lk:
+        terms.append(l_0 * (1 - z) % P)
+        terms.append(l_last * (z * z - z) % P)
+        terms.append((zn * (ap + beta) % P * (sp + gamma) - z * (a_c + beta) % P * (t_c + gamma)) * active % P)
+        terms.append(l_0 * (ap - sp) % P)
+        terms.append((ap - sp) * (ap - apm) % P * active % P)
+    return terms
+
+
+# (chunk, columns): no permutation; one full set; one set partly filled; 4 sets, the last partly filled; 3 sets, the last
+# partly filled; 16 sets of one column (the most a circuit may have)
+_PERM_SHAPES = [(2, 0), (3, 3), (4, 2), (2, 7), (5, 13), (1, 16)]
+
+
+def test_perm_set_products_match_big_int(shim):
+    rnd = random.Random(10)
+    P, k = o.P, 10
+    for chunk, ncols in _PERM_SHAPES[1:]:
+        cols, vals, sig = _perm_case(rnd, chunk, ncols)
+        for s in range((ncols + chunk - 1) // chunk):
+            beta, gamma, row = rnd.randrange(P), rnd.randrange(P), rnd.randrange(1 << k)
+            cd = beta * pow(o.DELTA_P, s * chunk, P) % P * pow(o.omega(k), row, P) % P   # beta delta^(s chunk) X, X = omega^row
+            out = (ctypes.c_uint8 * 64)()
+            shim.hs_perm_set(_ints([c[0] for c in cols]), _ints([c[1] for c in cols]), _fes(vals[0]), _fes(vals[1]), _fes(vals[2]), _fes(sig), s, chunk, ncols,
+                             _b32(beta), _b32(gamma), _b32(o.DELTA_P), _b32(cd), out)
+            with_sigma = with_id = 1
+            cur = cd
+            for c in range(s * chunk, min((s + 1) * chunk, ncols)):
+                v = vals[cols[c][0]][cols[c][1]]
+                with_sigma = with_sigma * (v + beta * sig[c] + gamma) % P
+                with_id = with_id * (v + cur + gamma) % P
+                cur = cur * o.DELTA_P % P
+            r = bytes(out)
+            assert (int.from_bytes(r[:32], "little"), int.from_bytes(r[32:], "little")) == (with_sigma, with_id), (chunk, ncols, s)
+
+
+def test_arg_fold_matches_big_int(shim):
+    rnd = random.Random(11)
+    P = o.P
+    for chunk, ncols in _PERM_SHAPES:
+        nsets = (ncols + chunk - 1) // chunk
+        for L in (0, 1, 2):
+            for _ in range(3):
+                cols, vals, sig = _perm_case(rnd, chunk, ncols)
+                pz = [[rnd.randrange(P) for _ in range(3)] for _ in range(nsets)]
+                lk = [[rnd.randrange(P) for _ in range(7)] for _ in range(L)]
+                acc, x, y, beta, gamma, l_0, l_last, active = (rnd.randrange(P) for _ in range(8))
+                out = (ctypes.c_uint8 * 32)()
+                shim.hs_arg_fold(_fes([acc, x, y, beta, gamma, l_0, l_last, active]), _b32(o.DELTA_P), _ints([c[0] for c in cols]), _ints([c[1] for c in cols]),
+                                 _fes(vals[0]), _fes(vals[1]), _fes(vals[2]), _fes(sig), _fes([v for z in pz for v in z]), nsets, chunk, ncols, L,
+                                 _fes([v for e in lk for v in e]), out)
+                terms = _ref_arg_terms(cols, vals, sig, pz, lk, x, beta, gamma, l_0, l_last, active, chunk)
+                want = acc
+                for t in terms:
+                    want = (want * y + t) % P
+                assert int.from_bytes(bytes(out), "little") == want, (chunk, ncols, L)
+                assert shim.hs_arg_terms(nsets, L) == len(terms)
