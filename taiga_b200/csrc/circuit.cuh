@@ -20,22 +20,17 @@ struct ProveWs { std::vector<DevMem<uint8_t>> blocks, tables; std::vector<std::v
 
 struct Circuit {
   const Srs* srs;
-  // deep copy of the description
   uint32_t k, na, nf, ni, degree, bf, P, L, chunk, nsets, pieces; int ext_k, R; size_t n, usable;
   std::vector<tb_query> aq, fq, iq; std::vector<tb_column> perm;
-  std::vector<tb_expr_node> nodes; std::vector<uint32_t> roots; std::vector<uint8_t> consts_bytes; uint32_t nconsts;
-  std::vector<std::vector<uint32_t>> lk_in, lk_tab;
+  std::vector<Fp> consts_host;   // the constants (Montgomery) the verifier's gate programs read; `consts` is the device copy
   Fp vk_repr;  // canonical
   // device tables
   DevMem<Fp> fixed_vals, fixed_polys, fixed_cosets, sig_vals, sig_polys, sig_cosets;
   DevMem<Fp> l0, l_last, l_blind, consts, wr_inv;
   DevMem<Fp> coset_pre;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
   DevMem<int2> d_perm;
+  // the programs of gate_plan (gates.cuh), host and device copies
   QProgram prog_lookups;
-  // gate programs in gate_nparts[big] parts, big = (batch size >= 8): small batches run more, shorter programs (latency), large
-  // ones fewer (less duplicated work).  `gate_parts` holds the constraints evaluated on every sub-coset (all of them when the
-  // circuit is not split), `gate_parts_lo` the low-degree ones (degree <= R / 2) that are evaluated on every second sub-coset only
-  static constexpr int gate_nparts[2] = {8, 4};
   std::vector<QProgram> gate_parts[2], gate_parts_lo[2];
   bool split = false; uint32_t num_constraints = 0, t_pl = 0;   // t_pl: permutation + lookup terms folded after the gates
   std::vector<Fp> t_inv; Fp delta, zeta, omega, r_inv;

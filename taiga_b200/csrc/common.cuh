@@ -25,7 +25,6 @@ struct ConstraintError : std::runtime_error { using std::runtime_error::runtime_
     if (_e != cudaSuccess)                                                                              \
       throw tb::CudaError(std::string(#expr) + " failed: " + cudaGetErrorString(_e) + " at " + __FILE__ + ":" + std::to_string(__LINE__)); \
   } while (0)
-#define TB_REQUIRE(cond, msg) do { if (!(cond)) throw std::invalid_argument(std::string(msg) + " (" #cond ")"); } while (0)
 
 // Owner of one device allocation that outlives a call (SRS, proving key, context tables, workspaces): cudaMalloc / cudaFree,
 // which no stream orders, since such an allocation may outlive the context whose stream made it.  DevBuf is the stream-ordered

@@ -9,12 +9,15 @@
 // Replaces (on device) pasta_curves `Fp`/`Fq` as used by halo2_proofs under taiga_halo2/src/proof.rs:33-40.
 #pragma once
 #include <cstdint>
+#include <stdexcept>
+#include <string>
 
 #ifdef __CUDACC__
 #define TB_HD __host__ __device__ __forceinline__
 #else
 #define TB_HD inline
 #endif
+#define TB_REQUIRE(cond, msg) do { if (!(cond)) throw std::invalid_argument(std::string(msg) + " (" #cond ")"); } while (0)
 
 namespace tb {
 

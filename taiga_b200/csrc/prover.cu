@@ -34,7 +34,7 @@ static void to_cosets(Ctx* ctx, const Circuit& C, const Fp* polys, Fp* cosets, F
 
 static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, const uint8_t* fixed, const uint8_t* sigma) {
   TB_REQUIRE(cs->k == srs->k, "circuit k must match the SRS");
-  TB_REQUIRE(cs->cs_degree >= 3 && cs->num_perm_columns <= PERM_MAX_SETS * (cs->cs_degree - 2), "unsupported constraint system shape");
+  gate_desc_check(cs);
   std::unique_ptr<Circuit> Cp(new Circuit());
   Circuit& C = *Cp;
   C.srs = srs;
@@ -50,43 +50,6 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   C.fq.assign(cs->fixed_queries, cs->fixed_queries + cs->num_fixed_queries);
   C.iq.assign(cs->instance_queries, cs->instance_queries + cs->num_instance_queries);
   C.perm.assign(cs->perm_columns, cs->perm_columns + C.P);
-  C.nodes.assign(cs->nodes, cs->nodes + cs->num_nodes);
-  C.roots.assign(cs->constraint_roots, cs->constraint_roots + cs->num_constraints);
-  C.nconsts = cs->num_constants;
-  C.consts_bytes.assign(cs->constants, cs->constants + 32 * (size_t)cs->num_constants);
-  for (uint32_t l = 0; l < C.L; ++l) {
-    TB_REQUIRE(cs->lookups && cs->lookups[l].num_exprs >= 1 && cs->lookups[l].input_roots && cs->lookups[l].table_roots, "a lookup needs at least one expression pair");
-    C.lk_in.emplace_back(cs->lookups[l].input_roots, cs->lookups[l].input_roots + cs->lookups[l].num_exprs);
-    C.lk_tab.emplace_back(cs->lookups[l].table_roots, cs->lookups[l].table_roots + cs->lookups[l].num_exprs);
-  }
-  for (auto& q : C.aq) TB_REQUIRE(q.column < C.na, "advice query column out of range");
-  for (auto& q : C.fq) TB_REQUIRE(q.column < C.nf, "fixed query column out of range");
-  for (auto& q : C.iq) TB_REQUIRE(q.column < C.ni, "instance query column out of range");
-  // the description comes across the ABI: reject anything that would make the expression compiler recurse without end or a
-  // kernel index out of bounds (forward references, cycles, stray constant / query / column indices)
-  for (size_t i = 0; i < C.nodes.size(); ++i) {
-    const tb_expr_node& nd = C.nodes[i];
-    TB_REQUIRE(nd.op <= TB_EX_SCALE, "bad expression node");
-    switch (nd.op) {
-      case TB_EX_CONST: TB_REQUIRE(nd.a < cs->num_constants, "expression constant index out of range"); break;
-      case TB_EX_ADVICE: TB_REQUIRE(nd.a < cs->num_advice_queries, "expression advice query index out of range"); break;
-      case TB_EX_FIXED: TB_REQUIRE(nd.a < cs->num_fixed_queries, "expression fixed query index out of range"); break;
-      case TB_EX_INSTANCE: TB_REQUIRE(nd.a < cs->num_instance_queries, "expression instance query index out of range"); break;
-      case TB_EX_NEG: TB_REQUIRE(nd.a < i, "expression nodes must be in topological order"); break;
-      case TB_EX_SCALE: TB_REQUIRE(nd.a < i && nd.b < cs->num_constants, "bad SCALE node"); break;
-      default: TB_REQUIRE(nd.a < i && nd.b < i, "expression nodes must be in topological order"); break;
-    }
-  }
-  for (uint32_t r : C.roots) TB_REQUIRE(r < C.nodes.size(), "constraint root out of range");
-  for (uint32_t l = 0; l < C.L; ++l) {
-    for (uint32_t r : C.lk_in[l]) TB_REQUIRE(r < C.nodes.size(), "lookup input root out of range");
-    for (uint32_t r : C.lk_tab[l]) TB_REQUIRE(r < C.nodes.size(), "lookup table root out of range");
-  }
-  for (auto& pc : C.perm) {
-    TB_REQUIRE(pc.kind <= TB_COL_INSTANCE, "permutation column kind out of range");
-    TB_REQUIRE(pc.index < (pc.kind == TB_COL_ADVICE ? C.na : pc.kind == TB_COL_FIXED ? C.nf : C.ni), "permutation column index out of range");
-  }
-  TB_REQUIRE(cs->blinding_factors >= 1 && cs->num_advice >= 1, "unsupported constraint system shape");
   memcpy(C.vk_repr.l, cs->vk_transcript_repr, 32);
 
   C.delta = delta_const<Fp>(); C.zeta = zeta_const<Fp>(); C.omega = omega_k<Fp>((int)C.k);
@@ -100,9 +63,8 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
 
   size_t n = C.n;
   // constants -> Montgomery
-  { std::vector<Fp> cm(C.nconsts);
-    for (uint32_t i = 0; i < C.nconsts; ++i) { Fp v; memcpy(v.l, C.consts_bytes.data() + 32 * i, 32); cm[i] = v.to_mont(); }
-    C.consts = DevMem<Fp>(cm); }
+  for (uint32_t i = 0; i < cs->num_constants; ++i) { Fp v; memcpy(v.l, cs->constants + 32 * (size_t)i, 32); C.consts_host.push_back(v.to_mont()); }
+  C.consts = DevMem<Fp>(C.consts_host);
   { std::vector<int2> pc; for (auto& c : C.perm) pc.push_back(make_int2((int)c.kind, (int)c.index)); C.d_perm = DevMem<int2>(pc); }
 
   { // per-element factors of the forward coset hooks (one multiplication per coefficient instead of up to two and a table walk);
@@ -137,31 +99,21 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
     TB_CUDA(cudaMemcpyAsync(C.l_blind.get(), lc.get() + 2 * (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->sync(); }
 
-  // expression programs (descriptor rebuilt from the deep copy so pointers stay valid)
-  { tb_cs_desc d = *cs;
-    C.num_constraints = cs->num_constraints;
-    C.t_pl = perm_lookup_terms(C.nsets, C.L);
-    // Degree split: a constraint of degree <= R / 2 is a polynomial of fewer than (R / 2) * n coefficients, so the sum of all such
-    // constraints is fixed by its values on every second sub-coset; only the high-degree constraints (and the permutation /
-    // lookup terms) need all R sub-cosets.  Worth it when the low class carries a good part of the arithmetic.
-    std::vector<int> deg = q_constraint_degrees(&d);
-    std::vector<uint32_t> all, lo, hi;
-    for (uint32_t j = 0; j < cs->num_constraints; ++j) { all.push_back(j); ((C.R >= 4 && deg[j] <= C.R / 2) ? lo : hi).push_back(j); }
-    { std::vector<QProgram> t_all, t_lo;
-      q_compile_gates_split(&d, all, 1, &t_all); q_compile_gates_split(&d, lo, 1, &t_lo);
-      C.split = tb_tune("TB_Q_SPLIT", 1) != 0 && C.R >= 4 && !lo.empty() && !hi.empty() && t_lo[0].ninstr * 10 >= t_all[0].ninstr * 3;
-      if (getenv("TB_DEBUG")) fprintf(stderr, "[tb] circuit k=%u degree=%u: %u constraints, %zu of degree <= %d (%d of %d instructions): split %s\n", C.k, C.degree, cs->num_constraints,
-                                      lo.size(), C.R / 2, t_lo[0].ninstr, t_all[0].ninstr, C.split ? "on" : "off"); }
+  // expression programs
+  { GatePlan g = gate_plan(cs, C.R, tb_tune("TB_Q_SPLIT", 1) != 0);
+    C.num_constraints = g.num_constraints; C.t_pl = g.t_pl; C.split = g.split;
     for (int big = 0; big < 2; ++big) {
-      q_compile_gates_split(&d, C.split ? hi : all, Circuit::gate_nparts[big], &C.gate_parts[big]);
-      if (C.split) q_compile_gates_split(&d, lo, Circuit::gate_nparts[big], &C.gate_parts_lo[big]);
+      for (auto& p : g.gate_parts[big]) C.gate_parts[big].emplace_back(std::move(p));
+      for (auto& p : g.gate_parts_lo[big]) C.gate_parts_lo[big].emplace_back(std::move(p));
     }
+    C.prog_lookups = QProgram(std::move(g.lookups));
     if (getenv("TB_DEBUG")) {
+      fprintf(stderr, "[tb] circuit k=%u degree=%u: %u constraints, %zu of degree <= %d (%d of %d instructions): split %s\n", C.k, C.degree, cs->num_constraints,
+              g.num_lo, C.R / 2, g.lo_instr, g.all_instr, C.split ? "on" : "off");
       for (auto* m : {C.gate_parts, C.gate_parts_lo})
         for (int big = 0; big < 2; ++big) if (!m[big].empty()) {
-          fprintf(stderr, "[tb]   %s %d parts:", m == C.gate_parts ? "all/high" : "low", Circuit::gate_nparts[big]); for (auto& qp : m[big]) fprintf(stderr, " %d/%d", qp.ninstr, qp.nregs); fprintf(stderr, "\n"); }
-    }
-    q_compile_lookups(&d, &C.prog_lookups); }
+          fprintf(stderr, "[tb]   %s %d parts:", m == C.gate_parts ? "all/high" : "low", GatePlan::nparts[big]); for (auto& qp : m[big]) fprintf(stderr, " %zu/%d", qp.prog.code.size(), qp.prog.nregs); fprintf(stderr, "\n"); }
+    } }
 
   // ---- evaluation section order (plonk/prover.rs) and multiopen query order
   int last_rot = -(int)(C.bf + 1);
@@ -504,7 +456,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       keep = ws.buf<Fp>((size_t)Rlo * B * NC * n); elo = ws.buf<Fp>((size_t)B * Rlo * n); vlo = ws.buf<Fp>((size_t)B * Rlo * n); clo = ws.buf<Fp>((size_t)B * Rlo * n);
       qlo = ws.buf<Fp>((size_t)B * Rlo * n); rlo_poly = ws.buf<Fp>((size_t)B * n); rlo_coset = ws.buf<Fp>((size_t)B * n);
       int gexp[Q_MAX_PARTS] = {0};
-      for (size_t p = 0; p < lprogs->size(); ++p) gexp[p] = J - 1 - (*lprogs)[p].last + (int)C.t_pl;
+      for (size_t p = 0; p < lprogs->size(); ++p) gexp[p] = J - 1 - (*lprogs)[p].prog.last + (int)C.t_pl;
       for (int kq = 0; kq < Rlo; ++kq) {
         const int k1 = 2 * kq;
         Fp* ck = keep.get() + (size_t)kq * B * NC * n;
@@ -524,7 +476,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       q_lo_split(ctx, clo.get(), (long long)Rlo * nn, Rlo, rlo_poly.get(), nn, qlo.get(), (long long)Rlo * nn, (int)n, B);
     }
     int gexp_hi[Q_MAX_PARTS] = {0};
-    for (size_t p = 0; p < gprogs.size(); ++p) gexp_hi[p] = J - 1 - gprogs[p].last;
+    for (size_t p = 0; p < gprogs.size(); ++p) gexp_hi[p] = J - 1 - gprogs[p].prog.last;
     for (int k1 = 0; k1 < R; ++k1) {
       NttHook<Fp> h = coset_hook(C, k1, false);
       Fp* ck = cosets.get();

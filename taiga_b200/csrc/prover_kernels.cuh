@@ -1,6 +1,7 @@
 // Declarations for lookup.cu and quotient.cu (kernel drivers used by prover.cu).
 #pragma once
 #include "argument.cuh"
+#include "gates.cuh"
 #include "prover.cuh"
 
 namespace tb {
@@ -11,29 +12,14 @@ void sort_keys(Ctx* c, Fp* keys, int n, int arrays);                            
 void lookup_arrange(Ctx* c, const Fp* sortedA, const Fp* sortedT, Fp* scratch, Fp* S, int n, int usable, int arrays, uint32_t* d_err);
 
 // ---------------------------------------------------------------- quotient.cu
-// Row-parallel expression interpreter (SURVEY.md App. E.6).  Temporaries live in a shared-memory register file laid
-// out [reg][thread] as two 16-byte halves; leaves (column queries, constants) are read straight from global memory.
-enum QOp { Q_MOV = 0, Q_NEG, Q_ADD, Q_SUB, Q_MUL, Q_FOLD_Y, Q_LK_BEGIN, Q_FOLD_A, Q_FOLD_S, Q_LK_STORE, Q_GBEGIN, Q_GFOLD, Q_GEND };
-enum QKind { K_REG = 0, K_ADV, K_FIX, K_INST, K_CONST };
-struct alignas(16) QInstr { uint32_t w0; uint32_t a, b, pad; };  // w0 = op | dst << 8 | akind << 16 | bkind << 24 (one 128-bit load)
-inline QInstr q_make(int op, int dst, int ak, uint32_t a, int bk, uint32_t b) { QInstr i; i.w0 = op | (dst << 8) | (ak << 16) | (bk << 24); i.a = a; i.b = b; i.pad = 0; return i; }
-
+// Row-parallel interpreter of the programs of gates.cuh.  Temporaries live in a shared-memory register file laid out
+// [reg][thread] as two 16-byte halves; leaves (column queries, constants) are read straight from global memory.
 struct QProgram {           // compiled once per circuit (host), resident on the device
-  std::vector<QInstr> host; int nregs = 0;
-  DevMem<QInstr> dev; int ninstr = 0;
-  int last = -1;            // index of the last constraint the program folds: its result is sum_j y^(last - j) e_j over its constraints
+  GateProgram prog; DevMem<QInstr> dev;
+  QProgram() {}
+  explicit QProgram(GateProgram&& p) : prog(std::move(p)) { if (!prog.code.empty()) dev = DevMem<QInstr>(prog.code); }
 };
-// Flattens the expression DAG reachable from `roots` into a register-allocated instruction list.
-// mode 0: gate constraints folded with y (Q_FOLD_Y per root);  mode 1: lookup compression (theta folds + stores)
-// The (sorted) constraint subset `subset` split into `parts` groups of similar cost, one program each (row-parallel AND
-// constraint-parallel evaluation).  Folds are gap-aware: program p yields S_p = sum_{j in p} y^(last_p - j) e_j, so any
-// set of programs combines as sum_p y^(J - 1 - last_p) S_p, whatever subset of the J constraints each one holds.
-constexpr int Q_MAX_PARTS = 8;
-void q_compile_gates_split(const tb_cs_desc* cs, const std::vector<uint32_t>& subset, int parts, std::vector<QProgram>* out);
-// polynomial degree of every constraint (a column query counts 1): decides which sub-cosets a constraint must be evaluated on
-std::vector<int> q_constraint_degrees(const tb_cs_desc* cs);
 struct QPartList { const QInstr* prog[Q_MAX_PARTS]; int ninstr[Q_MAX_PARTS]; int nparts; long long part_stride; };
-void q_compile_lookups(const tb_cs_desc* cs, QProgram* out);
 
 struct QData {
   const Fp* adv; long long adv_pstride;     // [B][num_advice][n]

@@ -50,25 +50,6 @@ __global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_
   ok[p] = s.is_inf() ? 1 : 0;
 }
 
-static Fp eval_expr(const Circuit& C, uint32_t root, std::vector<Fp>& memo, std::vector<char>& done, const std::vector<Fp>& adv, const std::vector<Fp>& fix,
-                    const std::vector<Fp>& inst) {
-  if (done[root]) return memo[root];
-  const tb_expr_node& nd = C.nodes[root];
-  Fp r;
-  switch (nd.op) {
-    case TB_EX_CONST: { Fp c; memcpy(c.l, C.consts_bytes.data() + 32 * nd.a, 32); r = c.to_mont(); break; }
-    case TB_EX_ADVICE: r = adv[nd.a]; break;
-    case TB_EX_FIXED: r = fix[nd.a]; break;
-    case TB_EX_INSTANCE: r = inst[nd.a]; break;
-    case TB_EX_NEG: r = eval_expr(C, nd.a, memo, done, adv, fix, inst).neg(); break;
-    case TB_EX_ADD: r = eval_expr(C, nd.a, memo, done, adv, fix, inst) + eval_expr(C, nd.b, memo, done, adv, fix, inst); break;
-    case TB_EX_MUL: r = eval_expr(C, nd.a, memo, done, adv, fix, inst) * eval_expr(C, nd.b, memo, done, adv, fix, inst); break;
-    default: { Fp c; memcpy(c.l, C.consts_bytes.data() + 32 * nd.b, 32); r = eval_expr(C, nd.a, memo, done, adv, fix, inst) * c.to_mont(); }
-  }
-  memo[root] = r; done[root] = 1;
-  return r;
-}
-
 // the proof's evaluations at x, as argument.cuh reads them
 struct EvalView {
   const Circuit& C; std::map<std::pair<PolyId, int>, Fp>& ev; int last_rot;
@@ -153,31 +134,30 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     if (!ok) continue;
     // evaluations, in the prover's order (C.evals)
     std::map<std::pair<PolyId, int>, Fp> ev;
-    std::vector<Fp> adv_ev, fix_ev, inst_ev;
     for (auto& e : C.evals) {
       Fp v; if (!tr.read_scalar(v)) { ok = false; break; }
       ev[{e.poly, e.rot}] = v;
     }
     if (!ok) continue;
-    for (auto& q : C.iq) inst_ev.push_back(ev[{{PK_INST, (int)q.column}, q.rotation}]);
-    for (auto& q : C.aq) adv_ev.push_back(ev[{{PK_ADV, (int)q.column}, q.rotation}]);
-    for (auto& q : C.fq) fix_ev.push_back(ev[{{PK_FIXED, (int)q.column}, q.rotation}]);
     // expected h(x)
     Fp xn = x; for (int i = 0; i < kk; ++i) xn = xn.sqr();
     auto l_at = [&](int rot) { Fp wi = rot_pow(rot); return (xn - one) * n_inv * wi * (x - wi).inv(); };
     Fp l_last = l_at(last_rot), l_blind = Fp::zero(), l_0 = l_at(0);
     for (int r = -bf; r <= -1; ++r) l_blind = l_blind + l_at(r);
-    std::vector<Fp> memo(C.nodes.size()); std::vector<char> done(C.nodes.size(), 0);
+    // the circuit's programs at x: the gates as the quotient combines its parts (sum_p y^(J - 1 - last_p) S_p), and the lookups
+    const int J = (int)C.num_constraints;
+    std::vector<Fp> ypow(J + C.t_pl + 2, one), lk_a(L), lk_t(L);
+    for (size_t i = 1; i < ypow.size(); ++i) ypow[i] = ypow[i - 1] * y;
+    auto at_x = [&](int kind, int col, int rot) { return ev[{{kind == K_ADV ? PK_ADV : kind == K_FIX ? PK_FIXED : PK_INST, col}, rot}]; };
+    PointMachine<decltype(at_x)> m{at_x, C.consts_host.data(), ypow.data(), theta, lk_a.data(), lk_t.data()};
     Fp acc = Fp::zero();
-    for (uint32_t r : C.roots) acc = acc * y + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
+    for (const auto* parts : {&C.gate_parts[0], &C.gate_parts_lo[0]})
+      for (const QProgram& qp : *parts) acc = acc + ypow[J - 1 - qp.prog.last] * m.run(qp.prog);
+    m.run(C.prog_lookups.prog);
     const ArgPoint at = {y, beta, gamma, l_0, l_last, one - (l_last + l_blind)};
     acc = perm_fold(acc, EvalView{C, ev, last_rot}, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
-    for (int l = 0; l < L; ++l) {
-      Fp a = Fp::zero(), t = Fp::zero();
-      for (uint32_t r : C.lk_in[l]) a = a * theta + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
-      for (uint32_t r : C.lk_tab[l]) t = t * theta + eval_expr(C, r, memo, done, adv_ev, fix_ev, inst_ev);
-      acc = lookup_fold(acc, at, ev[{{PK_LZ, l}, 0}], ev[{{PK_LZ, l}, 1}], ev[{{PK_LPIN, l}, 0}], ev[{{PK_LPIN, l}, -1}], ev[{{PK_LPTAB, l}, 0}], a, t);
-    }
+    for (int l = 0; l < L; ++l)
+      acc = lookup_fold(acc, at, ev[{{PK_LZ, l}, 0}], ev[{{PK_LZ, l}, 1}], ev[{{PK_LPIN, l}, 0}], ev[{{PK_LPIN, l}, -1}], ev[{{PK_LPTAB, l}, 0}], lk_a[l], lk_t[l]);
     ev[{{PK_H, 0}, 0}] = acc * (xn - one).inv();
     // ---- multiopen
     Fp x1 = tr.squeeze(), x2 = tr.squeeze();

@@ -1,7 +1,9 @@
-// Host instantiation of the product's __host__ __device__ field/curve arithmetic, transcript and argument terms
-// (taiga_b200/csrc/*.cuh), so the same source the kernels compile can be checked on a CPU-only box against the oracle.
+// Host instantiation of the product's __host__ __device__ field/curve arithmetic, transcript, argument terms and gate
+// programs (taiga_b200/csrc/*.cuh), so the same source the kernels compile can be checked on a CPU-only box against the oracle.
+#include <cstdio>
 #include <cstring>
 #include "../taiga_b200/csrc/argument.cuh"
+#include "../taiga_b200/csrc/gates.cuh"
 #include "../taiga_b200/csrc/transcript.cuh"
 using namespace tb;
 template <class F> static void fop(int op, const uint8_t* a, const uint8_t* b, uint8_t* o) {
@@ -86,4 +88,54 @@ void hs_arg_fold(const uint8_t* pt, const uint8_t* delta, const int* kind, const
   put(acc, out);
 }
 uint32_t hs_arg_terms(uint32_t nsets, uint32_t L) { return perm_lookup_terms(nsets, L); }
+}
+
+// ---------------------------------------------------------------- gates.cuh
+static GatePlan g_plan;   // the plan of the last hs_gate_plan
+extern "C" {
+// checks cs and plans its programs for R sub-cosets: 1, or 0 with the rejection's message in err
+int hs_gate_plan(const tb_cs_desc* cs, int R, int allow_split, char* err, int cap) {
+  try { gate_desc_check(cs); g_plan = gate_plan(cs, R, allow_split != 0); return 1; }
+  catch (const std::invalid_argument& e) { snprintf(err, cap, "%s", e.what()); return 0; }
+}
+int hs_gate_split() { return g_plan.split; }
+uint32_t hs_gate_t_pl() { return g_plan.t_pl; }
+static const std::vector<GateProgram>& programs(int which) { return which < 2 ? g_plan.gate_parts[which] : g_plan.gate_parts_lo[which - 2]; }
+// list `which` (0, 1: gate_parts[big]; 2, 3: gate_parts_lo[big]; 4: the lookup program): with p < 0 the number of programs,
+// else program p's instruction count, its code (4 words per instruction, up to cap instructions) and meta = [nregs, last]
+int hs_gate_program(int which, int p, uint32_t* code, int cap, int* meta) {
+  if (p < 0) return which == 4 ? 1 : (int)programs(which).size();
+  const GateProgram& g = which == 4 ? g_plan.lookups : programs(which)[p];
+  for (int i = 0; i < (int)g.code.size() && i < cap; ++i) memcpy(code + 4 * i, &g.code[i], 16);
+  meta[0] = g.nregs; meta[1] = g.last;
+  return (int)g.code.size();
+}
+// The planned programs at one point; adv / fix / inst hold one value per query of the description.  gate = sum_p
+// y^(J - 1 - last_p) S_p over gate_parts[big] and gate_parts_lo[big]; lk = [L][compressed inputs, table].  Returns the
+// number of leaves read that match no query.
+int hs_gate_eval(const tb_cs_desc* cs, int big, const uint8_t* adv, const uint8_t* fix, const uint8_t* inst, const uint8_t* y, const uint8_t* theta,
+                 uint8_t* gate, uint8_t* lk) {
+  std::vector<Fp> consts;
+  for (uint32_t i = 0; i < cs->num_constants; ++i) consts.push_back(fe(cs->constants + 32 * (size_t)i));
+  int unmatched = 0;
+  auto at = [&](int kind, int col, int rot) {
+    const tb_query* q = kind == K_ADV ? cs->advice_queries : kind == K_FIX ? cs->fixed_queries : cs->instance_queries;
+    const uint32_t nq = kind == K_ADV ? cs->num_advice_queries : kind == K_FIX ? cs->num_fixed_queries : cs->num_instance_queries;
+    const uint8_t* v = kind == K_ADV ? adv : kind == K_FIX ? fix : inst;
+    for (uint32_t i = 0; i < nq; ++i) if ((int)q[i].column == col && q[i].rotation == rot) return fe(v + 32 * (size_t)i);
+    ++unmatched; return Fp::zero();
+  };
+  const int J = (int)cs->num_constraints;
+  std::vector<Fp> ypow(J + g_plan.t_pl + 2, Fp::one()), a(cs->num_lookups), t(cs->num_lookups);
+  for (size_t i = 1; i < ypow.size(); ++i) ypow[i] = ypow[i - 1] * fe(y);
+  PointMachine<decltype(at)> m{at, consts.data(), ypow.data(), fe(theta), a.data(), t.data()};
+  Fp acc = Fp::zero();
+  for (const auto* parts : {&g_plan.gate_parts[big], &g_plan.gate_parts_lo[big]})
+    for (const GateProgram& p : *parts) acc = acc + ypow[J - 1 - p.last] * m.run(p);
+  m.run(g_plan.lookups);
+  put(acc, gate);
+  for (uint32_t l = 0; l < cs->num_lookups; ++l) { put(a[l], lk + 64 * l); put(t[l], lk + 64 * l + 32); }
+  return unmatched;
+}
+void hs_constraint_degrees(const tb_cs_desc* cs, int* out) { std::vector<int> d = q_constraint_degrees(cs); for (size_t j = 0; j < d.size(); ++j) out[j] = d[j]; }
 }
