@@ -1,7 +1,7 @@
 // Minimal C++ caller of the host-side mirror (include/taiga_b200.hpp): a one-gate PLONKish circuit
 //     q * (a * b - c) = 0,  public c            (k = 5, 3 advice + 1 instance + 1 selector, no lookups,
 // a, b, c, instance in the permutation with the identity wiring except c[0] <-> instance[0]), proved and verified with
-// Proof::create / Proof::verify as a Taiga caller would (proof.rs:25-54).  Field arithmetic for the key material comes
+// Proof::create / Proof::verify (through a VerifyingKey) as a Taiga caller would (proof.rs:25-54).  Field arithmetic for the key material comes
 // from the library's own header in host mode.  Without an H100 it must fail loudly: there is no CPU fallback (that path and
 // the build are what tests/test_abi.py checks; the proving path itself is covered through the same C ABI by tests/test_gpu_*.py).
 //
@@ -114,10 +114,14 @@ int main(int argc, char** argv) {
     std::array<uint8_t, 32> seed{};   // a real caller draws this from its RNG (proof.rs:30)
 
     Proof proof = Proof::create(pk, params, AdviceTable{advice.data()}, instance, seed);
-    proof.verify(pk, params, instance);
+    // a verifier holds the verifying key only: the constraint system and the commitments keygen_vk made
+    std::vector<PointBytes> fixed_commitments, sigma_commitments;
+    pk.commitments(fixed_commitments, sigma_commitments);
+    VerifyingKey vk(params, cs, fixed_commitments, sigma_commitments);
+    proof.verify(vk, params, instance);
     std::printf("proof of %zu bytes created and verified; kernels launched: %llu\n", proof.inner().size(), (unsigned long long)ctx.launch_count());
     instance[0][0] = seven;
-    try { proof.verify(pk, params, instance); std::printf("ERROR: wrong instance accepted\n"); return 2; }
+    try { proof.verify(vk, params, instance); std::printf("ERROR: wrong instance accepted\n"); return 2; }
     catch (const Error& e) { std::printf("wrong instance rejected: %s (%s)\n", e.what(), e.kind()); }
     return 0;
   } catch (const Error& e) {

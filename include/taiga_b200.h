@@ -59,6 +59,11 @@ tb_status tb_prof_work(tb_ctx* ctx, double* modmuls_out);
 tb_status tb_ntt(tb_ctx* ctx, int field, uint32_t logn, int inverse, int coset, uint32_t batch, const uint8_t* in, uint8_t* out);
 tb_status tb_msm(tb_ctx* ctx, int curve, size_t n, uint32_t batch, const uint8_t* scalars, const uint8_t* points,
                  uint32_t window_bits, uint8_t* out_points);
+/* tb_decompress decodes n compressed Vesta points (32 bytes each: x little-endian, the parity of y in bit 255, 32 zero
+ *          bytes = the identity; pasta_curves `GroupEncoding::from_bytes`) into n 64-byte affine points, one device thread
+ *          per point.  ok[i] = 0 (and out[i] = 64 zero bytes) when x >= q, x is off the curve, or x = 0 with the sign bit
+ *          set; these are the encodings the verifier rejects in a proof. */
+tb_status tb_decompress(tb_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok);
 
 /* ---- the same primitives over DEVICE memory owned by the caller (e.g. torch tensors).  Device field elements
  * are 32-byte Montgomery residues (R = 2^256); convert with tb_dev_{to,from}_mont.  Work is enqueued on the
@@ -143,6 +148,24 @@ tb_status tb_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const 
  * accepted.  instance / instance_len as in tb_prove_batch. */
 tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len,
                           const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out);
+
+/* ---- verifying key: Proof::verify(vk, params, instance) for a caller that holds the VerifyingKey only (a node checking
+ * partial transactions gets it inside ResourceLogicVerifyingInfo, taiga_api.rs:110).  tb_vk_load takes the circuit
+ * description and the two commitment lists of the vk, as 64-byte affine points in the format tb_pk_commitments writes
+ * (64 zero bytes = the identity):
+ *   fixed_commitments : num_fixed points (vk.fixed_commitments)
+ *   sigma_commitments : num_perm_columns points (vk.permutation.commitments)
+ * It checks the description as tb_circuit_load does, requires cs->k == the SRS's k, and refuses (TB_ERR_INVALID) a
+ * commitment with a coordinate >= q or off the curve.  A tb_vk holds host memory only (no per-row table) and refers to
+ * `srs`, which must outlive it.  tb_verify_batch_vk takes the arguments of tb_verify_batch, has its limits, and gives the
+ * same verdicts; every point of the batch is decoded on the device before the transcripts are replayed. */
+typedef struct tb_vk tb_vk;
+tb_status tb_vk_load(tb_ctx* ctx, const tb_srs* srs, const tb_cs_desc* cs, const uint8_t* fixed_commitments, const uint8_t* sigma_commitments,
+                     tb_vk** out);
+void tb_vk_free(tb_vk* vk);
+size_t tb_vk_proof_len(const tb_vk* vk);
+tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len,
+                             const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out);
 
 #ifdef __cplusplus
 }

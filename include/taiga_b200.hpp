@@ -134,12 +134,14 @@ struct ConstraintSystem {
 };
 
 // ProvingKey<vesta::Affine> (COMPLIANCE_PROVING_KEY / TRIVIAL_RESOURCE_LOGIC_PK): fixed and sigma polynomials, their
-// extended cosets and the compiled constraint programs, resident on the device.  Also what Proof::verify needs of the vk.
+// extended cosets and the compiled constraint programs, resident on the device.  Proof::verify also accepts it in place of
+// the VerifyingKey.
 class ProvingKey {
  public:
   // fixed_values: num_fixed x 2^k, sigma_values: perm_columns x 2^k field elements (Lagrange basis, column-major)
   ProvingKey(const Params& params, const ConstraintSystem& cs, const uint8_t* fixed_values, const uint8_t* sigma_values)
-      : params_(&params), num_advice_(cs.num_advice), num_instance_(cs.num_instance), k_(cs.k) {
+      : params_(&params), num_advice_(cs.num_advice), num_instance_(cs.num_instance), k_(cs.k), num_fixed_(cs.num_fixed),
+        num_perm_((uint32_t)cs.perm_columns.size()) {
     std::vector<tb_lookup> lk;
     tb_cs_desc d = cs.view(lk);
     tb_pk* p = nullptr;
@@ -152,12 +154,48 @@ class ProvingKey {
   uint32_t num_advice() const { return num_advice_; }
   uint32_t num_instance() const { return num_instance_; }
   size_t rows() const { return (size_t)1 << k_; }
+  // keygen_vk: vk.fixed_commitments and vk.permutation.commitments (constant.rs:150)
+  void commitments(std::vector<PointBytes>& fixed, std::vector<PointBytes>& sigma) const {
+    fixed.assign(num_fixed_, PointBytes{});
+    sigma.assign(num_perm_, PointBytes{});
+    params_->context().check(tb_pk_commitments(params_->context().get(), pk_.get(), fixed.empty() ? nullptr : fixed[0].data(),
+                                               sigma.empty() ? nullptr : sigma[0].data()));
+  }
 
  private:
   struct Del { void operator()(tb_pk* p) const { tb_pk_free(p); } };
   const Params* params_;
-  uint32_t num_advice_, num_instance_, k_;
+  uint32_t num_advice_, num_instance_, k_, num_fixed_, num_perm_;
   std::unique_ptr<tb_pk, Del> pk_;
+};
+
+// VerifyingKey<vesta::Affine> as Proof::verify uses it (proof.rs:45-54): the constraint system and the fixed and
+// permutation commitments, no proving-key table.  Built from what a verifier receives (ResourceLogicVerifyingInfo carries
+// the vk, taiga_api.rs:110); host memory only.
+class VerifyingKey {
+ public:
+  VerifyingKey(const Params& params, const ConstraintSystem& cs, const std::vector<PointBytes>& fixed_commitments,
+               const std::vector<PointBytes>& sigma_commitments)
+      : params_(&params), num_instance_(cs.num_instance) {
+    if (fixed_commitments.size() != cs.num_fixed || sigma_commitments.size() != cs.perm_columns.size())
+      throw Error(TB_ERR_INVALID, "one commitment per fixed and per permutation column is required");
+    std::vector<tb_lookup> lk;
+    tb_cs_desc d = cs.view(lk);
+    tb_vk* v = nullptr;
+    params.context().check(tb_vk_load(params.context().get(), params.get(), &d, fixed_commitments.empty() ? nullptr : fixed_commitments[0].data(),
+                                      sigma_commitments.empty() ? nullptr : sigma_commitments[0].data(), &v));
+    vk_.reset(v);
+  }
+  const tb_vk* get() const { return vk_.get(); }
+  const Params& params() const { return *params_; }
+  size_t proof_len() const { return tb_vk_proof_len(vk_.get()); }
+  uint32_t num_instance() const { return num_instance_; }
+
+ private:
+  struct Del { void operator()(tb_vk* v) const { tb_vk_free(v); } };
+  const Params* params_;
+  uint32_t num_instance_;
+  std::unique_ptr<tb_vk, Del> vk_;
 };
 
 // The witness of one proof: what `Circuit::synthesize` assigned (after batch_invert_assigned), num_advice x 2^k elements.
@@ -203,29 +241,45 @@ class Proof {
   }
 
   // Proof::verify (proof.rs:45-54): returns normally iff accepted, throws Error("ConstraintSystemFailure") otherwise --
-  // `Result<(), plonk::Error>` in the reference.
+  // `Result<(), plonk::Error>` in the reference.  `vk` is the VerifyingKey, or the ProvingKey of the circuit.
+  void verify(const VerifyingKey& vk, const Params& params, const std::vector<std::vector<FieldBytes>>& instance) const {
+    std::vector<bool> ok = verify_batch(vk, params, {*this}, {instance});
+    if (!ok[0]) throw Error(TB_ERR_CONSTRAINT, "proof rejected");
+  }
   void verify(const ProvingKey& vk, const Params& params, const std::vector<std::vector<FieldBytes>>& instance) const {
     std::vector<bool> ok = verify_batch(vk, params, {*this}, {instance});
     if (!ok[0]) throw Error(TB_ERR_CONSTRAINT, "proof rejected");
   }
+  static std::vector<bool> verify_batch(const VerifyingKey& vk, const Params& params, const std::vector<Proof>& proofs,
+                                        const std::vector<std::vector<std::vector<FieldBytes>>>& instances) {
+    return verify_with(params, proofs, instances, vk.num_instance(), [&](uint32_t n, const uint8_t* inst, const uint32_t* lens, const uint8_t* buf, size_t plen, uint8_t* ok) {
+      return tb_verify_batch_vk(params.context().get(), vk.get(), n, inst, lens, buf, plen, plen, ok);
+    });
+  }
   static std::vector<bool> verify_batch(const ProvingKey& vk, const Params& params, const std::vector<Proof>& proofs,
                                         const std::vector<std::vector<std::vector<FieldBytes>>>& instances) {
+    return verify_with(params, proofs, instances, vk.num_instance(), [&](uint32_t n, const uint8_t* inst, const uint32_t* lens, const uint8_t* buf, size_t plen, uint8_t* ok) {
+      return tb_verify_batch(params.context().get(), vk.get(), n, inst, lens, buf, plen, plen, ok);
+    });
+  }
+
+ private:
+  template <class Call>
+  static std::vector<bool> verify_with(const Params& params, const std::vector<Proof>& proofs, const std::vector<std::vector<std::vector<FieldBytes>>>& instances,
+                                       uint32_t num_instance, Call call) {
     const uint32_t n = (uint32_t)proofs.size();
     if (n == 0 || instances.size() != n) throw Error(TB_ERR_INVALID, "one instance per proof is required");
     std::vector<uint32_t> lens;
-    std::vector<uint8_t> inst = flatten(instances, vk.num_instance(), lens);
+    std::vector<uint8_t> inst = flatten(instances, num_instance, lens);
     const size_t plen = proofs[0].bytes_.size();
     std::vector<uint8_t> buf(plen * n), ok(n, 0);
     for (uint32_t i = 0; i < n; ++i) {
       if (proofs[i].bytes_.size() != plen) throw Error(TB_ERR_INVALID, "proofs of one circuit have one length");
       std::memcpy(buf.data() + i * plen, proofs[i].bytes_.data(), plen);
     }
-    const Context& ctx = params.context();
-    ctx.check(tb_verify_batch(ctx.get(), vk.get(), n, inst.data(), lens.data(), buf.data(), plen, plen, ok.data()));
+    params.context().check(call(n, inst.data(), lens.data(), buf.data(), plen, ok.data()));
     return std::vector<bool>(ok.begin(), ok.end());
   }
-
- private:
   // per proof the instance columns concatenated; every proof of a batch must use the same column lengths
   static std::vector<uint8_t> flatten(const std::vector<std::vector<std::vector<FieldBytes>>>& instances, uint32_t num_instance,
                                       std::vector<uint32_t>& lens) {

@@ -15,7 +15,7 @@ use pasta_curves::arithmetic::CurveAffine;
 use pasta_curves::{pallas, vesta};
 use rand_core::RngCore;
 
-use super::{Any, ConstraintSystem, Error, Expression, ProvingKey};
+use super::{Any, ConstraintSystem, Error, Expression, ProvingKey, VerifyingKey};
 use crate::poly::commitment::Params;
 use crate::poly::{LagrangeCoeff, Polynomial};
 use crate::transcript::{EncodedChallenge, TranscriptWrite};
@@ -139,6 +139,68 @@ impl Flat {
     }
 }
 
+/// Calls `f` with the tb_cs_desc of `vk.cs()` (the description is valid only inside the call: it points into locals).
+fn with_desc<R>(k: u32, vk: &VerifyingKey<vesta::Affine>, f: impl FnOnce(&tb::tb_cs_desc) -> R) -> R {
+    let cs: &ConstraintSystem<F> = vk.cs();
+    let q = |col: usize, rot: i32| tb::tb_query { column: col as u32, rotation: rot };
+    let aq: Vec<_> = cs.advice_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
+    let fq: Vec<_> = cs.fixed_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
+    let iq: Vec<_> = cs.instance_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
+    let perm: Vec<_> = cs
+        .permutation
+        .get_columns()
+        .iter()
+        .map(|c| tb::tb_column {
+            kind: match c.column_type() {
+                Any::Advice => tb::TB_COL_ADVICE,
+                Any::Fixed => tb::TB_COL_FIXED,
+                Any::Instance => tb::TB_COL_INSTANCE,
+            },
+            index: c.index() as u32,
+        })
+        .collect();
+    let mut flat = Flat::default();
+    let roots: Vec<u32> = cs.gates.iter().flat_map(|g| g.polynomials().iter()).map(|p| flat.expr(p)).collect();
+    let lk_roots: Vec<(Vec<u32>, Vec<u32>)> = cs
+        .lookups
+        .iter()
+        .map(|l| (l.input_expressions.iter().map(|e| flat.expr(e)).collect(), l.table_expressions.iter().map(|e| flat.expr(e)).collect()))
+        .collect();
+    let lookups: Vec<tb::tb_lookup> = lk_roots
+        .iter()
+        .map(|(i, t)| tb::tb_lookup { num_exprs: i.len() as u32, input_roots: i.as_ptr(), table_roots: t.as_ptr() })
+        .collect();
+    let consts: Vec<u8> = flat.consts.iter().flatten().copied().collect();
+    let mut repr = [0u8; 32];
+    repr.copy_from_slice(vk.transcript_repr.to_repr().as_ref());
+    let desc = tb::tb_cs_desc {
+        k,
+        num_advice: cs.num_advice_columns as u32,
+        num_fixed: cs.num_fixed_columns as u32,
+        num_instance: cs.num_instance_columns as u32,
+        cs_degree: cs.degree() as u32,
+        blinding_factors: cs.blinding_factors() as u32,
+        num_advice_queries: aq.len() as u32,
+        advice_queries: aq.as_ptr(),
+        num_fixed_queries: fq.len() as u32,
+        fixed_queries: fq.as_ptr(),
+        num_instance_queries: iq.len() as u32,
+        instance_queries: iq.as_ptr(),
+        num_perm_columns: perm.len() as u32,
+        perm_columns: perm.as_ptr(),
+        num_constants: flat.consts.len() as u32,
+        constants: consts.as_ptr(),
+        num_nodes: flat.nodes.len() as u32,
+        nodes: flat.nodes.as_ptr(),
+        num_constraints: roots.len() as u32,
+        constraint_roots: roots.as_ptr(),
+        num_lookups: lookups.len() as u32,
+        lookups: lookups.as_ptr(),
+        vk_transcript_repr: repr,
+    };
+    f(&desc)
+}
+
 /// Device-resident proving key of one circuit (COMPLIANCE_PROVING_KEY, constant.rs:145-152;
 /// TRIVIAL_RESOURCE_LOGIC_PK, resource_logic_examples.rs:50-61).
 pub struct GpuProvingKey {
@@ -153,62 +215,6 @@ impl GpuProvingKey {
     pub fn new(gp: &GpuParams, pk: &ProvingKey<vesta::Affine>) -> Result<Self, Error> {
         let cs: &ConstraintSystem<F> = pk.get_vk().cs();
         let n = 1usize << gp.k;
-        let q = |col: usize, rot: i32| tb::tb_query { column: col as u32, rotation: rot };
-        let aq: Vec<_> = cs.advice_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
-        let fq: Vec<_> = cs.fixed_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
-        let iq: Vec<_> = cs.instance_queries.iter().map(|(c, r)| q(c.index(), r.0)).collect();
-        let perm: Vec<_> = cs
-            .permutation
-            .get_columns()
-            .iter()
-            .map(|c| tb::tb_column {
-                kind: match c.column_type() {
-                    Any::Advice => tb::TB_COL_ADVICE,
-                    Any::Fixed => tb::TB_COL_FIXED,
-                    Any::Instance => tb::TB_COL_INSTANCE,
-                },
-                index: c.index() as u32,
-            })
-            .collect();
-        let mut flat = Flat::default();
-        let roots: Vec<u32> = cs.gates.iter().flat_map(|g| g.polynomials().iter()).map(|p| flat.expr(p)).collect();
-        let lk_roots: Vec<(Vec<u32>, Vec<u32>)> = cs
-            .lookups
-            .iter()
-            .map(|l| (l.input_expressions.iter().map(|e| flat.expr(e)).collect(), l.table_expressions.iter().map(|e| flat.expr(e)).collect()))
-            .collect();
-        let lookups: Vec<tb::tb_lookup> = lk_roots
-            .iter()
-            .map(|(i, t)| tb::tb_lookup { num_exprs: i.len() as u32, input_roots: i.as_ptr(), table_roots: t.as_ptr() })
-            .collect();
-        let consts: Vec<u8> = flat.consts.iter().flatten().copied().collect();
-        let mut repr = [0u8; 32];
-        repr.copy_from_slice(pk.get_vk().transcript_repr.to_repr().as_ref());
-        let desc = tb::tb_cs_desc {
-            k: gp.k,
-            num_advice: cs.num_advice_columns as u32,
-            num_fixed: cs.num_fixed_columns as u32,
-            num_instance: cs.num_instance_columns as u32,
-            cs_degree: cs.degree() as u32,
-            blinding_factors: cs.blinding_factors() as u32,
-            num_advice_queries: aq.len() as u32,
-            advice_queries: aq.as_ptr(),
-            num_fixed_queries: fq.len() as u32,
-            fixed_queries: fq.as_ptr(),
-            num_instance_queries: iq.len() as u32,
-            instance_queries: iq.as_ptr(),
-            num_perm_columns: perm.len() as u32,
-            perm_columns: perm.as_ptr(),
-            num_constants: flat.consts.len() as u32,
-            constants: consts.as_ptr(),
-            num_nodes: flat.nodes.len() as u32,
-            nodes: flat.nodes.as_ptr(),
-            num_constraints: roots.len() as u32,
-            constraint_roots: roots.as_ptr(),
-            num_lookups: lookups.len() as u32,
-            lookups: lookups.as_ptr(),
-            vk_transcript_repr: repr,
-        };
         let col_bytes = |cols: &[Polynomial<F, LagrangeCoeff>]| -> Vec<u8> {
             cols.iter().flat_map(|c| c.iter().flat_map(|v| v.to_repr().as_ref().to_vec())).collect()
         };
@@ -217,12 +223,41 @@ impl GpuProvingKey {
         debug_assert_eq!(fixed.len(), cs.num_fixed_columns * n * 32);
         let mut out = std::ptr::null_mut();
         let ctx = gp.ctx.lock().unwrap();
-        let st = unsafe { tb::tb_circuit_load(*ctx, gp.srs, &desc, fixed.as_ptr(), sigma.as_ptr(), &mut out) };
+        let st = with_desc(gp.k, pk.get_vk(), |desc| unsafe { tb::tb_circuit_load(*ctx, gp.srs, desc, fixed.as_ptr(), sigma.as_ptr(), &mut out) });
         if st != 0 {
             eprintln!("tb_circuit_load: {}", last_error(*ctx));
             return Err(Error::Synthesis);
         }
         Ok(GpuProvingKey { pk: out, proof_len: unsafe { tb::tb_pk_proof_len(out) }, num_advice: cs.num_advice_columns })
+    }
+}
+
+/// The verifying key of one circuit on the host (what `Proof::verify` takes, proof.rs:45-54): built from a
+/// `VerifyingKey` alone, e.g. the one inside `ResourceLogicVerifyingInfo` (taiga_api.rs:110), with no proving key.
+pub struct GpuVerifyingKey {
+    vk: *mut tb::tb_vk,
+}
+unsafe impl Send for GpuVerifyingKey {}
+unsafe impl Sync for GpuVerifyingKey {}
+
+impl GpuVerifyingKey {
+    pub fn new(gp: &GpuParams, vk: &VerifyingKey<vesta::Affine>) -> Result<Self, Error> {
+        let fixed: Vec<u8> = vk.fixed_commitments().iter().flat_map(affine_bytes).collect();
+        let sigma: Vec<u8> = vk.permutation().commitments().iter().flat_map(affine_bytes).collect();
+        let mut out = std::ptr::null_mut();
+        let ctx = gp.ctx.lock().unwrap();
+        let st = with_desc(gp.k, vk, |desc| unsafe { tb::tb_vk_load(*ctx, gp.srs, desc, fixed.as_ptr(), sigma.as_ptr(), &mut out) });
+        if st != 0 {
+            eprintln!("tb_vk_load: {}", last_error(*ctx));
+            return Err(Error::Synthesis);
+        }
+        Ok(GpuVerifyingKey { vk: out })
+    }
+}
+
+impl Drop for GpuVerifyingKey {
+    fn drop(&mut self) {
+        unsafe { tb::tb_vk_free(self.vk) }
     }
 }
 
@@ -297,8 +332,8 @@ pub fn create_proofs_gpu(
 /// COMPLIANCE_PROVING_KEY (constant.rs:128-152).
 pub fn _doc_anchor() {}
 
-/// `Proof::verify` for many proofs of one circuit (shielded_ptx.rs:137-153 loops them one by one, 35 ms each on CPU).
-pub fn verify_batch_gpu(gp: &GpuParams, gpk: &GpuProvingKey, instances: &[&[&[F]]], proofs: &[&[u8]]) -> Result<Vec<bool>, Error> {
+/// The instance columns of every proof, concatenated, and the column lengths (those of the first proof).
+fn flatten_instances(instances: &[&[&[F]]]) -> (Vec<u8>, Vec<u32>) {
     let inst_len: Vec<u32> = instances[0].iter().map(|c| c.len() as u32).collect();
     let mut inst = Vec::new();
     for proof in instances {
@@ -308,13 +343,34 @@ pub fn verify_batch_gpu(gp: &GpuParams, gpk: &GpuProvingKey, instances: &[&[&[F]
             }
         }
     }
+    (inst, inst_len)
+}
+
+/// Runs one of the two batched verifiers (`call` gets ctx, n, instance, instance_len, proofs, proof_len, ok).
+fn verify_with(
+    gp: &GpuParams,
+    instances: &[&[&[F]]],
+    proofs: &[&[u8]],
+    call: impl FnOnce(*mut tb::tb_ctx, u32, *const u8, *const u32, *const u8, usize, *mut u8) -> i32,
+) -> Result<Vec<bool>, Error> {
+    let (inst, inst_len) = flatten_instances(instances);
     let plen = proofs[0].len();
     let flat: Vec<u8> = proofs.iter().flat_map(|p| p.iter().copied()).collect();
     let mut ok = vec![0u8; proofs.len()];
     let ctx = gp.ctx.lock().unwrap();
-    let st = unsafe { tb::tb_verify_batch(*ctx, gpk.pk, proofs.len() as u32, inst.as_ptr(), inst_len.as_ptr(), flat.as_ptr(), plen, plen, ok.as_mut_ptr()) };
+    let st = call(*ctx, proofs.len() as u32, inst.as_ptr(), inst_len.as_ptr(), flat.as_ptr(), plen, ok.as_mut_ptr());
     if st != 0 {
         return Err(map_status(st, *ctx));
     }
     Ok(ok.into_iter().map(|b| b == 1).collect())
+}
+
+/// `Proof::verify` for many proofs of one circuit (shielded_ptx.rs:137-153 loops them one by one, 35 ms each on CPU).
+pub fn verify_batch_gpu(gp: &GpuParams, gpk: &GpuProvingKey, instances: &[&[&[F]]], proofs: &[&[u8]]) -> Result<Vec<bool>, Error> {
+    verify_with(gp, instances, proofs, |ctx, n, inst, lens, flat, plen, ok| unsafe { tb::tb_verify_batch(ctx, gpk.pk, n, inst, lens, flat, plen, plen, ok) })
+}
+
+/// The same verdicts from the verifying key alone: what a node that checks partial transactions holds.
+pub fn verify_batch_gpu_vk(gp: &GpuParams, gvk: &GpuVerifyingKey, instances: &[&[&[F]]], proofs: &[&[u8]]) -> Result<Vec<bool>, Error> {
+    verify_with(gp, instances, proofs, |ctx, n, inst, lens, flat, plen, ok| unsafe { tb::tb_verify_batch_vk(ctx, gvk.vk, n, inst, lens, flat, plen, plen, ok) })
 }

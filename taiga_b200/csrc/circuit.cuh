@@ -1,4 +1,6 @@
-// The device-resident proving key of one circuit (tb_pk) shared by prover.cu and verifier.cu.
+// What the prover and the verifier know of one circuit: its shape (host only, derived from the tb_cs_desc), the
+// device-resident proving key built on it (tb_pk), and the verifying key (tb_vk: the shape plus the fixed and sigma
+// commitments).  Shared by shape.cu, prover.cu and verifier.cu.
 #pragma once
 #include <atomic>
 #include <map>
@@ -18,33 +20,42 @@ struct QueryRef { PolyId poly; int rot; };
 // with the SAME context and batch size while a call is in flight is refused (TB_ERR_INVALID) instead of corrupting it.
 struct ProveWs { std::vector<DevMem<uint8_t>> blocks, tables; std::vector<std::vector<uint8_t>> table_bytes; std::atomic<int> busy{0}; };
 
-struct Circuit {
-  const Srs* srs;
+// Everything the description fixes, built once by shape_build: sizes, domain constants, the compiled programs and the
+// order of the proof's elements.  Host memory only and nothing per row, so a verifying key costs kilobytes.
+struct Shape {
   uint32_t k, na, nf, ni, degree, bf, P, L, chunk, nsets, pieces; int ext_k, R; size_t n, usable;
   std::vector<tb_query> aq, fq, iq; std::vector<tb_column> perm;
-  std::vector<Fp> consts_host;   // the constants (Montgomery) the verifier's gate programs read; `consts` is the device copy
+  std::vector<Fp> consts_host;   // the constants (Montgomery) the gate programs read
   Fp vk_repr;  // canonical
-  // device tables
-  DevMem<Fp> fixed_vals, fixed_polys, fixed_cosets, sig_vals, sig_polys, sig_cosets;
-  DevMem<Fp> l0, l_last, l_blind, consts, wr_inv;
-  DevMem<Fp> coset_pre;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
-  DevMem<int2> d_perm;
-  // the programs of gate_plan (gates.cuh), host and device copies
-  QProgram prog_lookups;
-  std::vector<QProgram> gate_parts[2], gate_parts_lo[2];
-  bool split = false; uint32_t num_constraints = 0, t_pl = 0;   // t_pl: permutation + lookup terms folded after the gates
+  GatePlan plan;                 // the programs of gate_plan (gates.cuh)
   std::vector<Fp> t_inv; Fp delta, zeta, omega, r_inv;
   Fp delta_c0[PERM_MAX_SETS];
-  // evaluation / multiopen structure (host)
+  // evaluation / multiopen structure
   std::vector<QueryRef> evals;            // transcript order of the evaluation section
   std::vector<QueryRef> queries;          // multiopen query order
   std::vector<int> rots;                  // distinct rotations (evaluation points), in order of first appearance in `queries`
   std::vector<PolyId> uniq; std::vector<int> uniq_set; std::vector<std::vector<int>> point_sets;
   uint32_t proof_len;
+  std::vector<uint32_t> point_offsets;    // byte offset of every point of a proof, in transcript order
+};
+// checks the description (gate_desc_check, k == srs_k) and derives its shape; `allow_split`: the quotient's degree split
+Shape shape_build(const tb_cs_desc* cs, uint32_t srs_k, bool allow_split);
+
+struct Circuit : Shape {
+  const Srs* srs;
+  // device tables
+  DevMem<Fp> fixed_vals, fixed_polys, fixed_cosets, sig_vals, sig_polys, sig_cosets;
+  DevMem<Fp> l0, l_last, l_blind, consts, wr_inv;
+  DevMem<Fp> coset_pre;   // [R][n]: zeta^(i mod 3) * w_ext^(i * k1), the factor the forward coset NTT applies to coefficient i for sub-coset k1
+  DevMem<int2> d_perm;
+  // the programs of `plan` with their device copies
+  QProgram prog_lookups;
+  std::vector<QProgram> gate_parts[2], gate_parts_lo[2];
   // persistent per-batch-size workspace and cached small tables (see prove_batch)
   mutable std::mutex mu;                                                   // guards the two caches below
   mutable std::map<std::pair<const Ctx*, int>, std::unique_ptr<ProveWs>> ws;
   mutable std::vector<Aff<Fq>> vk_fixed, vk_sigma;   // verifying-key commitments (Montgomery, host), filled on first verification
+  explicit Circuit(Shape&& s) : Shape(std::move(s)) {}
   // the workspace of (context, batch size), marked busy; nullptr if a call is already using it.  Claiming under the lock
   // lets release_idle() free every workspace that is not marked.
   ProveWs* claim_workspace(const Ctx* c, int B) const {
@@ -68,6 +79,13 @@ struct Circuit {
     TB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
     TB_CUDA(cudaMemPoolTrimTo(pool, 0));
   }
+};
+
+// tb_vk: what Proof::verify needs of a circuit.  The commitments are Montgomery affine points, the identity (0, 0).
+struct VerifyingKey {
+  Shape shape;
+  const Srs* srs;
+  std::vector<Aff<Fq>> fixed, sigma;
 };
 
 }  // namespace tb

@@ -33,37 +33,14 @@ static void to_cosets(Ctx* ctx, const Circuit& C, const Fp* polys, Fp* cosets, F
 }
 
 static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, const uint8_t* fixed, const uint8_t* sigma) {
-  TB_REQUIRE(cs->k == srs->k, "circuit k must match the SRS");
-  gate_desc_check(cs);
-  std::unique_ptr<Circuit> Cp(new Circuit());
+  std::unique_ptr<Circuit> Cp(new Circuit(shape_build(cs, srs->k, tb_tune("TB_Q_SPLIT", 1) != 0)));
   Circuit& C = *Cp;
   C.srs = srs;
-  C.k = cs->k; C.n = size_t(1) << C.k; C.na = cs->num_advice; C.nf = cs->num_fixed; C.ni = cs->num_instance; C.degree = cs->cs_degree; C.bf = cs->blinding_factors;
-  TB_REQUIRE(C.n > C.bf + 2, "too few rows");
-  C.usable = C.n - (C.bf + 1);
-  C.P = cs->num_perm_columns; C.L = cs->num_lookups; C.chunk = C.degree - 2; C.nsets = C.P ? (C.P + C.chunk - 1) / C.chunk : 0;
-  C.pieces = C.degree - 1;
-  C.ext_k = C.k; while ((size_t(1) << C.ext_k) < C.n * C.pieces) C.ext_k++;
-  TB_REQUIRE(C.ext_k <= TW_LOG, "extended domain too large");
-  C.R = 1 << (C.ext_k - C.k);
-  C.aq.assign(cs->advice_queries, cs->advice_queries + cs->num_advice_queries);
-  C.fq.assign(cs->fixed_queries, cs->fixed_queries + cs->num_fixed_queries);
-  C.iq.assign(cs->instance_queries, cs->instance_queries + cs->num_instance_queries);
-  C.perm.assign(cs->perm_columns, cs->perm_columns + C.P);
-  memcpy(C.vk_repr.l, cs->vk_transcript_repr, 32);
-
-  C.delta = delta_const<Fp>(); C.zeta = zeta_const<Fp>(); C.omega = omega_k<Fp>((int)C.k);
-  C.r_inv = Fp::from_u32((uint32_t)C.R).inv();
-  for (int s = 0; s < PERM_MAX_SETS; ++s) C.delta_c0[s] = C.delta.pow_u64((uint64_t)s * C.chunk);
-  Fp w_ext = omega_k<Fp>(C.ext_k);
-  { Fp zn = C.zeta.pow_u64(C.n), step = w_ext.pow_u64(C.n), cur = zn;
-    for (int k1 = 0; k1 < C.R; ++k1) { C.t_inv.push_back((cur - Fp::one()).inv()); cur = cur * step; }
+  { Fp step = omega_k<Fp>(C.ext_k).pow_u64(C.n);
     std::vector<Fp> wr(C.R); Fp wri = step.inv(); wr[0] = Fp::one(); for (int e = 1; e < C.R; ++e) wr[e] = wr[e - 1] * wri;
     C.wr_inv = DevMem<Fp>(wr); }
 
   size_t n = C.n;
-  // constants -> Montgomery
-  for (uint32_t i = 0; i < cs->num_constants; ++i) { Fp v; memcpy(v.l, cs->constants + 32 * (size_t)i, 32); C.consts_host.push_back(v.to_mont()); }
   C.consts = DevMem<Fp>(C.consts_host);
   { std::vector<int2> pc; for (auto& c : C.perm) pc.push_back(make_int2((int)c.kind, (int)c.index)); C.d_perm = DevMem<int2>(pc); }
 
@@ -99,67 +76,20 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
     TB_CUDA(cudaMemcpyAsync(C.l_blind.get(), lc.get() + 2 * (size_t)C.R * n, sz, cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->sync(); }
 
-  // expression programs
-  { GatePlan g = gate_plan(cs, C.R, tb_tune("TB_Q_SPLIT", 1) != 0);
-    C.num_constraints = g.num_constraints; C.t_pl = g.t_pl; C.split = g.split;
-    for (int big = 0; big < 2; ++big) {
-      for (auto& p : g.gate_parts[big]) C.gate_parts[big].emplace_back(std::move(p));
-      for (auto& p : g.gate_parts_lo[big]) C.gate_parts_lo[big].emplace_back(std::move(p));
-    }
-    C.prog_lookups = QProgram(std::move(g.lookups));
-    if (getenv("TB_DEBUG")) {
-      fprintf(stderr, "[tb] circuit k=%u degree=%u: %u constraints, %zu of degree <= %d (%d of %d instructions): split %s\n", C.k, C.degree, cs->num_constraints,
-              g.num_lo, C.R / 2, g.lo_instr, g.all_instr, C.split ? "on" : "off");
-      for (auto* m : {C.gate_parts, C.gate_parts_lo})
-        for (int big = 0; big < 2; ++big) if (!m[big].empty()) {
-          fprintf(stderr, "[tb]   %s %d parts:", m == C.gate_parts ? "all/high" : "low", GatePlan::nparts[big]); for (auto& qp : m[big]) fprintf(stderr, " %zu/%d", qp.prog.code.size(), qp.prog.nregs); fprintf(stderr, "\n"); }
-    } }
-
-  // ---- evaluation section order (plonk/prover.rs) and multiopen query order
-  int last_rot = -(int)(C.bf + 1);
-  for (auto& q : C.iq) C.evals.push_back({{PK_INST, (int)q.column}, q.rotation});
-  for (auto& q : C.aq) C.evals.push_back({{PK_ADV, (int)q.column}, q.rotation});
-  for (auto& q : C.fq) C.evals.push_back({{PK_FIXED, (int)q.column}, q.rotation});
-  C.evals.push_back({{PK_RANDOM, 0}, 0});
-  for (uint32_t c = 0; c < C.P; ++c) C.evals.push_back({{PK_SIG, (int)c}, 0});
-  for (uint32_t s = 0; s < C.nsets; ++s) {
-    C.evals.push_back({{PK_PZ, (int)s}, 0}); C.evals.push_back({{PK_PZ, (int)s}, 1});
-    if (s + 1 < C.nsets) C.evals.push_back({{PK_PZ, (int)s}, last_rot});
+  // the programs of the shape, uploaded
+  const GatePlan& g = C.plan;
+  for (int big = 0; big < 2; ++big) {
+    for (auto& p : g.gate_parts[big]) C.gate_parts[big].emplace_back(GateProgram(p));
+    for (auto& p : g.gate_parts_lo[big]) C.gate_parts_lo[big].emplace_back(GateProgram(p));
   }
-  for (uint32_t l = 0; l < C.L; ++l) {
-    C.evals.push_back({{PK_LZ, (int)l}, 0}); C.evals.push_back({{PK_LZ, (int)l}, 1}); C.evals.push_back({{PK_LPIN, (int)l}, 0});
-    C.evals.push_back({{PK_LPIN, (int)l}, -1}); C.evals.push_back({{PK_LPTAB, (int)l}, 0});
+  C.prog_lookups = QProgram(GateProgram(g.lookups));
+  if (getenv("TB_DEBUG")) {
+    fprintf(stderr, "[tb] circuit k=%u degree=%u: %u constraints, %zu of degree <= %d (%d of %d instructions): split %s\n", C.k, C.degree, cs->num_constraints,
+            g.num_lo, C.R / 2, g.lo_instr, g.all_instr, g.split ? "on" : "off");
+    for (auto* m : {C.gate_parts, C.gate_parts_lo})
+      for (int big = 0; big < 2; ++big) if (!m[big].empty()) {
+        fprintf(stderr, "[tb]   %s %d parts:", m == C.gate_parts ? "all/high" : "low", GatePlan::nparts[big]); for (auto& qp : m[big]) fprintf(stderr, " %zu/%d", qp.prog.code.size(), qp.prog.nregs); fprintf(stderr, "\n"); }
   }
-  for (auto& q : C.iq) C.queries.push_back({{PK_INST, (int)q.column}, q.rotation});
-  for (auto& q : C.aq) C.queries.push_back({{PK_ADV, (int)q.column}, q.rotation});
-  for (uint32_t s = 0; s < C.nsets; ++s) { C.queries.push_back({{PK_PZ, (int)s}, 0}); C.queries.push_back({{PK_PZ, (int)s}, 1}); }
-  for (int s = (int)C.nsets - 1; s >= 0; --s) if (s + 1 < (int)C.nsets) C.queries.push_back({{PK_PZ, s}, last_rot});
-  for (uint32_t l = 0; l < C.L; ++l) {
-    C.queries.push_back({{PK_LZ, (int)l}, 0}); C.queries.push_back({{PK_LPIN, (int)l}, 0}); C.queries.push_back({{PK_LPTAB, (int)l}, 0});
-    C.queries.push_back({{PK_LPIN, (int)l}, -1}); C.queries.push_back({{PK_LZ, (int)l}, 1});
-  }
-  for (auto& q : C.fq) C.queries.push_back({{PK_FIXED, (int)q.column}, q.rotation});
-  for (uint32_t c = 0; c < C.P; ++c) C.queries.push_back({{PK_SIG, (int)c}, 0});
-  C.queries.push_back({{PK_H, 0}, 0});
-  C.queries.push_back({{PK_RANDOM, 0}, 0});
-  // multiopen::construct_intermediate_sets (points identified by rotation; sets ordered by first appearance)
-  { std::map<int, int> point_index; std::vector<std::set<int>> prots;
-    for (auto& q : C.queries) {
-      if (!point_index.count(q.rot)) { int idx = (int)point_index.size(); point_index[q.rot] = idx; C.rots.push_back(q.rot); }
-      size_t pos = 0; for (; pos < C.uniq.size(); ++pos) if (C.uniq[pos] == q.poly) break;
-      if (pos == C.uniq.size()) { C.uniq.push_back(q.poly); prots.emplace_back(); }
-      prots[pos].insert(point_index[q.rot]);
-    }
-    std::map<std::set<int>, int> set_index;
-    for (size_t c = 0; c < C.uniq.size(); ++c) {
-      if (!set_index.count(prots[c])) { int idx = (int)set_index.size(); set_index[prots[c]] = idx; }
-      C.uniq_set.push_back(set_index[prots[c]]);
-    }
-    C.point_sets.resize(set_index.size());
-    for (auto& kv : set_index) for (int pi : kv.first) C.point_sets[kv.second].push_back(C.rots[pi]); }
-  for (auto& e : C.evals) if (std::find(C.rots.begin(), C.rots.end(), e.rot) == C.rots.end()) C.rots.push_back(e.rot);
-  uint32_t commits = C.na + 3 * C.L + C.nsets + 1 + C.pieces;
-  C.proof_len = 32 * (commits + (uint32_t)C.evals.size() + 1 + (uint32_t)C.point_sets.size() + 1 + 2 * C.k + 2);
   return Cp.release();
 }
 
@@ -285,7 +215,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   const int V_QBLIND = va.one(nps), V_P_BLIND = va.one(), V_S_BLIND = va.one(), V_F = va.one();
   const int V_S_AT = va.one(), V_V = va.one(), V_LR = va.one(), V_RR = va.one(), V_VL = va.one(), V_VR = va.one();
   const int V_U = va.one(), V_UINV = va.one(), V_T0 = va.one(), V_C = va.one();
-  const int YTAB = (int)(C.num_constraints + C.t_pl) + 2;
+  const int YTAB = (int)(C.plan.num_constraints + C.plan.t_pl) + 2;
   const int V_YTAB = va.one(YTAB);   // y^i, 0 <= i < YTAB: gap-aware folds of the gate programs and the weights that combine them
   const int NV = va.next;
   WBuf<Fp> vars = ws.buf<Fp>((size_t)B * NV);
@@ -440,23 +370,23 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   // fewer live temporaries per part = smaller shared-memory register file = higher occupancy (ncu: 6 warps/SM with one
   // 26-register program vs 20 warps/SM with eight <=11-register parts), for ~15% more instructions in total.
   const std::vector<QProgram>& gprogs = C.gate_parts[B >= 8];
-  const std::vector<QProgram>* lprogs = C.split ? &C.gate_parts_lo[B >= 8] : nullptr;
+  const std::vector<QProgram>* lprogs = C.plan.split ? &C.gate_parts_lo[B >= 8] : nullptr;
   { Prog p; p.op(S_CONST, V_YTAB, 0, 0, 0); p.op(S_COPY, V_YTAB + 1, V_Y);
     for (int i = 2; i < YTAB; ++i) p.op(S_MUL, V_YTAB + i, V_YTAB + i - 1, V_Y);
     run_prog(p); }
-  const int J = (int)C.num_constraints;
+  const int J = (int)C.plan.num_constraints;
   WBuf<Fp> hext = ws.buf<Fp>((size_t)B * R * n), hcoef = ws.buf<Fp>((size_t)B * C.pieces * n);
   { WBuf<Fp> c_lkA = ws.buf<Fp>((size_t)B * L1 * n), c_lkS = ws.buf<Fp>((size_t)B * L1 * n), gate = ws.buf<Fp>((size_t)Q_MAX_PARTS * B * n), V = ws.buf<Fp>((size_t)B * R * n);
-    const int Rlo = C.split ? R / 2 : 0;
+    const int Rlo = C.plan.split ? R / 2 : 0;
     // ---- low-degree constraints: every second sub-coset only.  Their sum H_lo is interpolated (Rlo * n coefficients) and divided by
     // X^n - 1 in coefficient form, H_lo = q_lo (X^n - 1) + r_lo; q_lo goes straight into h, r_lo (n coefficients) joins the numerator
     // of the high-degree part as one more polynomial on every sub-coset.  The column cosets computed here are kept for the second pass.
     WBuf<Fp> keep, elo, vlo, clo, qlo, rlo_poly, rlo_coset;
-    if (C.split) {
+    if (C.plan.split) {
       keep = ws.buf<Fp>((size_t)Rlo * B * NC * n); elo = ws.buf<Fp>((size_t)B * Rlo * n); vlo = ws.buf<Fp>((size_t)B * Rlo * n); clo = ws.buf<Fp>((size_t)B * Rlo * n);
       qlo = ws.buf<Fp>((size_t)B * Rlo * n); rlo_poly = ws.buf<Fp>((size_t)B * n); rlo_coset = ws.buf<Fp>((size_t)B * n);
       int gexp[Q_MAX_PARTS] = {0};
-      for (size_t p = 0; p < lprogs->size(); ++p) gexp[p] = J - 1 - (*lprogs)[p].prog.last + (int)C.t_pl;
+      for (size_t p = 0; p < lprogs->size(); ++p) gexp[p] = J - 1 - (*lprogs)[p].prog.last + (int)C.plan.t_pl;
       for (int kq = 0; kq < Rlo; ++kq) {
         const int k1 = 2 * kq;
         Fp* ck = keep.get() + (size_t)kq * B * NC * n;
@@ -480,9 +410,9 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
     for (int k1 = 0; k1 < R; ++k1) {
       NttHook<Fp> h = coset_hook(C, k1, false);
       Fp* ck = cosets.get();
-      if (C.split && (k1 & 1) == 0) ck = keep.get() + (size_t)(k1 / 2) * B * NC * n;   // computed in the first pass
+      if (C.plan.split && (k1 & 1) == 0) ck = keep.get() + (size_t)(k1 / 2) * B * NC * n;   // computed in the first pass
       else ntt_run<Fp>(ctx, k, false, polys.get(), ck, scratch.get(), B * NC, nn, nn, &h, nullptr);
-      if (C.split) ntt_run<Fp>(ctx, k, false, rlo_poly.get(), rlo_coset.get(), scratch.get(), B, nn, nn, &h, nullptr);
+      if (C.plan.split) ntt_run<Fp>(ctx, k, false, rlo_poly.get(), rlo_coset.get(), scratch.get(), B, nn, nn, &h, nullptr);
       Fp* const c_adv = ck + (size_t)O_ADV * n; Fp* const c_inst = ck + (size_t)O_INST * n; Fp* const c_pz = ck + (size_t)O_PZ * n;
       Fp* const c_lz = ck + (size_t)O_LZ * n; Fp* const c_lpin = ck + (size_t)O_LPIN * n; Fp* const c_lptab = ck + (size_t)O_LPTAB * n;
       qd.adv = c_adv; qd.adv_pstride = PS; qd.inst = c_inst; qd.inst_pstride = PS;
@@ -492,7 +422,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       if (L) { qd.gate_out = nullptr; q_run(ctx, C.prog_lookups, qd, B); }
       QFinish f; memset(&f, 0, sizeof(f));
       f.gate = gate.get(); f.nparts = (int)gprogs.size(); f.gate_part_stride = (long long)B * nn; f.ytab_slot = V_YTAB; memcpy(f.gexp, gexp_hi, sizeof(gexp_hi));
-      f.rlo = C.split ? rlo_coset.get() : nullptr; f.rlo_pstride = nn;
+      f.rlo = C.plan.split ? rlo_coset.get() : nullptr; f.rlo_pstride = nn;
       f.adv = c_adv; f.adv_pstride = PS; f.inst = c_inst; f.inst_pstride = PS;
       f.fix = C.fixed_cosets.get(); f.sig = C.sig_cosets.get(); f.R = R; f.k1 = k1; f.l0 = C.l0.get(); f.l_last = C.l_last.get(); f.l_blind = C.l_blind.get();
       f.pz = c_pz; f.pz_pstride = PS; f.lz = c_lz; f.lpin = c_lpin; f.lptab = c_lptab; f.lk_pstride = PS; f.lkc_pstride = (long long)L1 * nn;
@@ -508,7 +438,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
       ntt_run<Fp>(ctx, k, true, hext.get() + (size_t)k1 * n, V.get() + (size_t)k1 * n, scratch.get(), B, (long long)R * nn, (long long)R * nn, nullptr, &h);
     }
     h_cross(ctx, V.get(), (long long)R * nn, hcoef.get(), (long long)C.pieces * nn, (int)n, R, (int)C.pieces, C.wr_inv.get(), 1, C.r_inv, C.zeta.sqr(), B);
-    if (C.split) q_add_blocks(ctx, hcoef.get(), (long long)C.pieces * nn, qlo.get(), (long long)Rlo * nn, Rlo - 1, (int)n, B);   // + H_lo div (X^n - 1)
+    if (C.plan.split) q_add_blocks(ctx, hcoef.get(), (long long)C.pieces * nn, qlo.get(), (long long)Rlo * nn, Rlo - 1, (int)n, B);   // + H_lo div (X^n - 1)
   }
   prf_fill(ctx, seed, proof0, R_H_BLIND, 0, VP(V_H_BLINDS), NV, 1, (int)C.pieces, B);
   poly_copy(ctx, blinds.get(), C.pieces, VP(V_H_BLINDS), NV, C.pieces, B);

@@ -130,14 +130,14 @@ TB_HD void compress_point(const Aff<Fq>& p, uint32_t* out) {
 }
 
 // 32 LE bytes -> Montgomery form; false unless the value is below the modulus
-template <class F> inline bool canonical(const uint8_t* b, F& out) {
+template <class F> TB_HD bool canonical(const uint8_t* b, F& out) {
   F raw; memcpy(raw.l, b, 32);
   F m; for (int i = 0; i < 8; ++i) m.l[i] = F::modulus_limb(i);
   if (F::cmp_raw(raw, m) >= 0) return false;
   out = raw.to_mont(); return true;
 }
 // square root in Fq (2-adicity 32) by Tonelli-Shanks; false if a is not a square
-inline bool tonelli_shanks(const Fq& a, Fq& out) {
+TB_HD bool tonelli_shanks(const Fq& a, Fq& out) {
   if (a.is_zero()) { out = a; return true; }
   uint32_t q[8]; for (int i = 0; i < 8; ++i) q[i] = Fq::modulus_limb(i);
   q[0] -= 1;                                    // m - 1 = 2^32 * odd
@@ -156,8 +156,9 @@ inline bool tonelli_shanks(const Fq& a, Fq& out) {
   }
   out = r; return true;
 }
-// the inverse of compress_point; false for x >= q, an x off the curve, and x = 0 with the sign bit set (5 is not a square)
-inline bool decompress_point(const uint8_t* b, Aff<Fq>& out) {
+// the inverse of compress_point; false for x >= q, an x off the curve, and x = 0 with the sign bit set (5 is not a square).
+// The verifier decodes a batch's points with it on the device (decompress_kernel, verifier.cu).
+TB_HD bool decompress_point(const uint8_t* b, Aff<Fq>& out) {
   uint8_t t[32]; memcpy(t, b, 32);
   int sign = t[31] >> 7; t[31] &= 0x7f;
   bool allz = true; for (int i = 0; i < 32; ++i) allz &= (t[i] == 0);

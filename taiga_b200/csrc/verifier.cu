@@ -16,17 +16,40 @@
 
 namespace tb {
 
-// the transcript replayed over the bytes of one proof; `bad` once a read failed or the identity was absorbed
+// One thread per point: the 32 bytes at in + (i / npts) * stride + off[i % npts] (off = nullptr: at in + stride * i), decoded
+// as decompress_point decodes them.  out[i] = the point in Montgomery form (the identity for 32 zero bytes), ok[i] = 1 iff
+// the encoding is canonical and on the curve (out[i] = the identity otherwise).
+__global__ void decompress_kernel(const uint8_t* __restrict__ in, size_t stride, const uint32_t* __restrict__ off, int npts, size_t count,
+                                  Aff<Fq>* __restrict__ out, uint8_t* __restrict__ ok) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const uint8_t* b = off ? in + (i / npts) * stride + off[i % npts] : in + stride * i;
+  Aff<Fq> p;
+  bool good = decompress_point(b, p);
+  out[i] = good ? p.to_mont() : Aff<Fq>::inf();
+  ok[i] = good ? 1 : 0;
+}
+static void decompress(Ctx* ctx, const uint8_t* d_in, size_t stride, const uint32_t* d_off, int npts, size_t count, Aff<Fq>* d_out, uint8_t* d_ok) {
+  if (!count) return;
+  ProfScope scope(ctx, PC_TRANSCRIPT);
+  launch(ctx, decompress_kernel, (unsigned)((count + 127) / 128), 128, 0, d_in, stride, d_off, npts, count, d_out, d_ok);
+}
+
+// the transcript replayed over the bytes of one proof; `bad` once a read failed or the identity was absorbed.  The points
+// were decoded before the replay (pts / pts_ok: this proof's points in transcript order, at the offsets `offsets`).
 struct VTranscript : Transcript {
   const uint8_t* rd; size_t len, pos = 0; bool bad = false;
-  VTranscript(const uint8_t* p, size_t n, const Fp& vk_repr) : rd(p), len(n) { start(vk_repr); }
+  const Aff<Fq>* pts; const uint8_t* pts_ok; const std::vector<uint32_t>& offsets; size_t ipt = 0;
+  VTranscript(const uint8_t* p, size_t n, const Fp& vk_repr, const Aff<Fq>* pts, const uint8_t* pts_ok, const std::vector<uint32_t>& offsets)
+      : rd(p), len(n), pts(pts), pts_ok(pts_ok), offsets(offsets) { start(vk_repr); }
   void common_point(const Aff<Fq>& p) { if (!absorb_point(p.from_mont())) bad = true; }
   bool read_point(Aff<Fq>& p) {
-    Aff<Fq> c;
-    if (pos + 32 > len || !decompress_point(rd + pos, c)) { bad = true; return false; }
-    pos += 32;
-    if (!absorb_point(c)) bad = true;
-    p = c.to_mont(); return !bad;
+    if (pos + 32 > len || ipt >= offsets.size()) { bad = true; return false; }
+    if (offsets[ipt] != pos) throw std::logic_error("internal error: proof point offsets");
+    if (!pts_ok[ipt]) { bad = true; return false; }
+    p = pts[ipt++]; pos += 32;
+    if (!absorb_point(p.from_mont())) bad = true;
+    return !bad;
   }
   bool read_scalar(Fp& s) {
     if (pos + 32 > len || !canonical<Fp>(rd + pos, s)) { bad = true; return false; }
@@ -52,7 +75,7 @@ __global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_
 
 // the proof's evaluations at x, as argument.cuh reads them
 struct EvalView {
-  const Circuit& C; std::map<std::pair<PolyId, int>, Fp>& ev; int last_rot;
+  const Shape& C; std::map<std::pair<PolyId, int>, Fp>& ev; int last_rot;
   Fp perm_col(int c) const { const tb_column& col = C.perm[c]; return ev[{{col.kind == TB_COL_ADVICE ? PK_ADV : col.kind == TB_COL_FIXED ? PK_FIXED : PK_INST, (int)col.index}, 0}]; }
   Fp sigma(int c) const { return ev[{{PK_SIG, c}, 0}]; }
   Fp z(int s) const { return ev[{{PK_PZ, s}, 0}]; }
@@ -60,28 +83,24 @@ struct EvalView {
   Fp z_last(int s) const { return ev[{{PK_PZ, s}, last_rot}]; }
 };
 
-static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride,
-                         size_t proof_len, uint8_t* ok_out) {
-  const Srs& srs = *C.srs;
+// n_proofs proofs of the circuit of shape C, whose fixed / sigma commitments are `vk_fixed` / `vk_sigma` (Montgomery)
+static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
+                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
   const size_t n = C.n; const int kk = (int)C.k, na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf, nf = C.nf, pieces = C.pieces;
   cudaStream_t st = ctx->stream;
-  size_t inst_total = 0; for (int c = 0; c < ni; ++c) inst_total += instance_len[c];
+  size_t inst_total = 0;
+  for (int c = 0; c < ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); inst_total += instance_len[c]; }
   for (int p = 0; p < K; ++p) ok_out[p] = 0;
-  // ---- verifying-key commitments (computed once per circuit, cached)
-  std::unique_lock<std::mutex> vk_lock(C.mu);
-  if (C.vk_fixed.size() != (size_t)nf || C.vk_sigma.size() != (size_t)P) {
-    for (int which = 0; which < 2; ++which) {
-      int cnt = which ? P : nf;
-      std::vector<Aff<Fq>>& dst = which ? C.vk_sigma : C.vk_fixed;
-      dst.assign(cnt, Aff<Fq>::inf());
-      if (!cnt) continue;
-      DevBuf<Fp> ones(ctx, cnt); DevBuf<Aff<Fq>> pts(ctx, cnt);
-      std::vector<Fp> h(cnt, Fp::one()); ones.upload(h.data(), cnt);
-      srs.commit(ctx, true, which ? C.sig_vals.get() : C.fixed_vals.get(), (long long)n, cnt, ones.get(), pts.get());
-      pts.download(dst.data(), cnt); ctx->sync();
-    }
-  }
-  vk_lock.unlock();
+  if (proof_len != C.proof_len) return;   // no proof of this length is accepted
+  // ---- every point of the batch, decoded on the device: [K][npts]
+  const int npts = (int)C.point_offsets.size();
+  std::vector<Aff<Fq>> dec((size_t)K * npts);
+  std::vector<uint8_t> dec_ok((size_t)K * npts);
+  { DevBuf<uint8_t> d_proofs(ctx, (size_t)K * proof_len), d_ok(ctx, dec_ok.size()); DevBuf<uint32_t> d_off(ctx, npts); DevBuf<Aff<Fq>> d_pts(ctx, dec.size());
+    TB_CUDA(cudaMemcpy2DAsync(d_proofs.get(), proof_len, proofs, proof_stride, proof_len, K, cudaMemcpyHostToDevice, st));
+    d_off.upload(C.point_offsets.data(), npts);
+    decompress(ctx, d_proofs.get(), proof_len, d_off.get(), npts, dec.size(), d_pts.get(), d_ok.get());
+    d_pts.download(dec.data(), dec.size()); d_ok.download(dec_ok.data(), dec_ok.size()); ctx->sync(); }
   // ---- instance commitments for the whole batch: commit_lagrange(instance, Blind::default())
   std::vector<Aff<Fq>> inst_comm((size_t)K * std::max(1, ni), Aff<Fq>::inf());
   if (ni) {
@@ -89,7 +108,6 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     iv.zero();
     size_t off = 0;
     for (int c = 0; c < ni; ++c) {
-      TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge");
       if (instance_len[c])
         TB_CUDA(cudaMemcpy2DAsync(iv.get() + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, K, cudaMemcpyHostToDevice, st));
       off += instance_len[c];
@@ -111,7 +129,7 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
   Fp omega = C.omega, omega_inv = C.omega.inv(), n_inv = Fp::from_u32((uint32_t)n).inv();
   auto rot_pow = [&](int rot) { Fp r = one; const Fp& w = rot >= 0 ? omega : omega_inv; for (int i = 0; i < std::abs(rot); ++i) r = r * w; return r; };
   for (int p = 0; p < K; ++p) {
-    VTranscript tr(proofs + (size_t)p * proof_stride, proof_len, C.vk_repr);
+    VTranscript tr(proofs + (size_t)p * proof_stride, proof_len, C.vk_repr, dec.data() + (size_t)p * npts, dec_ok.data() + (size_t)p * npts, C.point_offsets);
     bool ok = true;
     const uint8_t* ib = instance + 32 * inst_total * p;
     for (size_t i = 0; i < inst_total && ok; ++i) { Fp t; ok = canonical<Fp>(ib + 32 * i, t); }
@@ -145,15 +163,15 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     Fp l_last = l_at(last_rot), l_blind = Fp::zero(), l_0 = l_at(0);
     for (int r = -bf; r <= -1; ++r) l_blind = l_blind + l_at(r);
     // the circuit's programs at x: the gates as the quotient combines its parts (sum_p y^(J - 1 - last_p) S_p), and the lookups
-    const int J = (int)C.num_constraints;
-    std::vector<Fp> ypow(J + C.t_pl + 2, one), lk_a(L), lk_t(L);
+    const int J = (int)C.plan.num_constraints;
+    std::vector<Fp> ypow(J + C.plan.t_pl + 2, one), lk_a(L), lk_t(L);
     for (size_t i = 1; i < ypow.size(); ++i) ypow[i] = ypow[i - 1] * y;
     auto at_x = [&](int kind, int col, int rot) { return ev[{{kind == K_ADV ? PK_ADV : kind == K_FIX ? PK_FIXED : PK_INST, col}, rot}]; };
     PointMachine<decltype(at_x)> m{at_x, C.consts_host.data(), ypow.data(), theta, lk_a.data(), lk_t.data()};
     Fp acc = Fp::zero();
-    for (const auto* parts : {&C.gate_parts[0], &C.gate_parts_lo[0]})
-      for (const QProgram& qp : *parts) acc = acc + ypow[J - 1 - qp.prog.last] * m.run(qp.prog);
-    m.run(C.prog_lookups.prog);
+    for (const auto* parts : {&C.plan.gate_parts[0], &C.plan.gate_parts_lo[0]})
+      for (const GateProgram& g : *parts) acc = acc + ypow[J - 1 - g.last] * m.run(g);
+    m.run(C.plan.lookups);
     const ArgPoint at = {y, beta, gamma, l_0, l_last, one - (l_last + l_blind)};
     acc = perm_fold(acc, EvalView{C, ev, last_rot}, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
     for (int l = 0; l < L; ++l)
@@ -207,8 +225,8 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
     for (size_t c = 0; c < C.uniq.size(); ++c) {
       const PolyId& id = C.uniq[c]; Fp coef = coef_in_set[id] * x4pow[nps - 1 - C.uniq_set[c]];
       if (id.kind == PK_H) { Fp cur = coef; for (int i = 0; i < pieces; ++i) { push(hpts[i], cur); cur = cur * xn; } }
-      else if (id.kind == PK_FIXED) push(C.vk_fixed[id.idx], coef);
-      else if (id.kind == PK_SIG) push(C.vk_sigma[id.idx], coef);
+      else if (id.kind == PK_FIXED) push(vk_fixed[id.idx], coef);
+      else if (id.kind == PK_SIG) push(vk_sigma[id.idx], coef);
       else push(comm[id], coef);
     }
     push(q_prime, x4pow[nps]);
@@ -236,15 +254,93 @@ static void verify_batch(Ctx* ctx, const Circuit& C, int K, const uint8_t* insta
   for (int p = 0; p < K; ++p) ok_out[p] = (alive[p] && hok[p]) ? 1 : 0;
 }
 
+// The verifying key of a proving key: commit_lagrange(column, Blind::default()) of every fixed and sigma column, computed on
+// first use and kept with the key.
+static const Circuit& pk_commitments(Ctx* ctx, const Circuit& C) {
+  std::lock_guard<std::mutex> vk_lock(C.mu);
+  if (C.vk_fixed.size() != (size_t)C.nf || C.vk_sigma.size() != (size_t)C.P) {
+    for (int which = 0; which < 2; ++which) {
+      int cnt = which ? (int)C.P : (int)C.nf;
+      std::vector<Aff<Fq>>& dst = which ? C.vk_sigma : C.vk_fixed;
+      dst.assign(cnt, Aff<Fq>::inf());
+      if (!cnt) continue;
+      DevBuf<Fp> ones(ctx, cnt); DevBuf<Aff<Fq>> pts(ctx, cnt);
+      std::vector<Fp> h(cnt, Fp::one()); ones.upload(h.data(), cnt);
+      C.srs->commit(ctx, true, which ? C.sig_vals.get() : C.fixed_vals.get(), (long long)C.n, cnt, ones.get(), pts.get());
+      pts.download(dst.data(), cnt); ctx->sync();
+    }
+  }
+  return C;
+}
+
+// cnt commitments of 64 bytes (canonical affine x || y, 64 zero bytes = the identity) -> Montgomery points; refuses a
+// coordinate >= q and a point off the curve
+static std::vector<Aff<Fq>> parse_commitments(const uint8_t* b, size_t cnt, const char* what) {
+  std::vector<Aff<Fq>> out(cnt, Aff<Fq>::inf());
+  for (size_t i = 0; i < cnt; ++i, b += 64) {
+    bool zero = true; for (int j = 0; j < 64; ++j) zero &= b[j] == 0;
+    if (zero) continue;
+    Aff<Fq> p;
+    TB_REQUIRE(canonical<Fq>(b, p.x) && canonical<Fq>(b + 32, p.y), std::string(what) + " commitment " + std::to_string(i) + ": a coordinate is not below q");
+    TB_REQUIRE(p.y.sqr() == p.x.sqr() * p.x + Fq::from_u32(5), std::string(what) + " commitment " + std::to_string(i) + " is not on the curve");
+    out[i] = p;
+  }
+  return out;
+}
+
 }  // namespace tb
 
 using namespace tb;
-extern "C" tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs,
-                                     size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
+extern "C" {
+
+tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs,
+                          size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
   TB_API_BEGIN(ctx)
   const Circuit* C = reinterpret_cast<const Circuit*>(pk);
   TB_REQUIRE(C && n_proofs >= 1 && n_proofs <= 4096 && proofs && ok_out && proof_stride >= proof_len && (C->ni == 0 || (instance && instance_len)), "tb_verify_batch arguments");
   TB_CUDA(cudaSetDevice(ctx->c.device));
-  verify_batch(&ctx->c, *C, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
+  pk_commitments(&ctx->c, *C);
+  verify_batch(&ctx->c, *C, *C->srs, C->vk_fixed, C->vk_sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
   TB_API_END(ctx)
 }
+
+tb_status tb_vk_load(tb_ctx* ctx, const tb_srs* srs_, const tb_cs_desc* cs, const uint8_t* fixed_commitments, const uint8_t* sigma_commitments, tb_vk** out) {
+  TB_API_BEGIN(ctx)
+  const Srs* srs = reinterpret_cast<const Srs*>(srs_);
+  TB_REQUIRE(srs && cs && out && (fixed_commitments || cs->num_fixed == 0) && (sigma_commitments || cs->num_perm_columns == 0), "tb_vk_load arguments");
+  // the verifier combines the gate programs the same way whether the quotient's degree split is on or not
+  std::unique_ptr<VerifyingKey> vk(new VerifyingKey{shape_build(cs, srs->k, true), srs, {}, {}});
+  vk->fixed = parse_commitments(fixed_commitments, vk->shape.nf, "fixed");
+  vk->sigma = parse_commitments(sigma_commitments, vk->shape.P, "sigma");
+  *out = reinterpret_cast<tb_vk*>(vk.release());
+  TB_API_END(ctx)
+}
+void tb_vk_free(tb_vk* vk) { delete reinterpret_cast<VerifyingKey*>(vk); }
+size_t tb_vk_proof_len(const tb_vk* vk) { return vk ? reinterpret_cast<const VerifyingKey*>(vk)->shape.proof_len : 0; }
+
+tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs,
+                             size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
+  TB_API_BEGIN(ctx)
+  const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
+  TB_REQUIRE(vk && n_proofs >= 1 && n_proofs <= 4096 && proofs && ok_out && proof_stride >= proof_len && (vk->shape.ni == 0 || (instance && instance_len)),
+             "tb_verify_batch_vk arguments");
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  verify_batch(&ctx->c, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
+  TB_API_END(ctx)
+}
+
+tb_status tb_decompress(tb_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok) {
+  TB_API_BEGIN(ctx)
+  TB_REQUIRE(in && out && ok && n >= 1, "tb_decompress arguments");
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  Ctx* c = &ctx->c;
+  DevBuf<uint8_t> d_in(c, 32 * n), d_ok(c, n); DevBuf<Aff<Fq>> d_out(c, n);
+  d_in.upload(in, 32 * n);
+  decompress(c, d_in.get(), 32, nullptr, 1, n, d_out.get(), d_ok.get());
+  fe_from_mont<Fq>(c, reinterpret_cast<Fq*>(d_out.get()), 2 * n);
+  d_out.download(out, n); d_ok.download(ok, n);
+  c->sync();
+  TB_API_END(ctx)
+}
+
+}  // extern "C"

@@ -57,6 +57,11 @@ _SIGS = {
     "tb_pk_commitments": (_i, [_vp, _vp, _vp, _vp]),
     "tb_prove_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _sz]),
     "tb_verify_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
+    "tb_decompress": (_i, [_vp, _sz, _vp, _vp, _vp]),
+    "tb_vk_load": (_i, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
+    "tb_vk_free": (None, [_vp]),
+    "tb_vk_proof_len": (_sz, [_vp]),
+    "tb_verify_batch_vk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
 }
 
 
@@ -169,6 +174,16 @@ class Context:
         self._check(self._lib.tb_msm(self._h, curve, n, batch, _ptr(s), _ptr(p), window_bits, _ptr(out)))
         return out
 
+    def decompress(self, encodings):
+        """Compressed Vesta points [n, 32] -> (affine points uint8 [n, 64], accepted bool [n]); a rejected encoding gives
+        64 zero bytes, and so does the identity (32 zero bytes), which is accepted."""
+        e = _u8(encodings).reshape(-1, 32)
+        n = e.shape[0]
+        out = np.zeros((n, 64), np.uint8)
+        ok = np.zeros(n, np.uint8)
+        self._check(self._lib.tb_decompress(self._h, n, _ptr(e), _ptr(out), _ptr(ok)))
+        return out, ok.astype(bool)
+
     # ---- device-buffer primitives (torch tensors / raw device pointers)
     def dev_to_mont(self, field, t, n):
         self._check(self._lib.tb_dev_to_mont(self._h, field, _ptr(t), n))
@@ -208,6 +223,11 @@ class Srs:
 
     def load_circuit(self, keydata):
         return ProvingKey(self, keydata)
+
+    def load_verifying_key(self, keydata, fixed, sigma):
+        """VerifyingKey from the circuit description of `keydata` and the vk's commitments: fixed [num_fixed, 64],
+        sigma [num_perm_columns, 64] (what ProvingKey.commitments() returns).  keydata.fixed / keydata.sigma are not read."""
+        return VerifyingKey(self, keydata, fixed, sigma)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -267,20 +287,60 @@ class ProvingKey:
 
     def verify_batch(self, instance, instance_len, proofs, ctx=None):
         """Proof::verify for a batch: proofs = list of byte strings; returns a list of booleans."""
-        ctx = ctx or self.ctx
-        B = len(proofs)
-        plen = len(proofs[0])
-        assert all(len(p) == plen for p in proofs)
-        buf = np.frombuffer(b"".join(proofs), np.uint8).copy()
-        inst = _u8(instance)
-        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
-        ok = np.zeros(B, np.uint8)
-        ctx._check(ctx._lib.tb_verify_batch(ctx._h, self._h, B, _ptr(inst), _ptr(lens), _ptr(buf), plen, plen, _ptr(ok)))
-        return [bool(v) for v in ok]
+        return _verify_batch(ctx or self.ctx, "tb_verify_batch", self._h, instance, instance_len, proofs)
+
+    def verifying_key(self):
+        """The VerifyingKey of this circuit, built from commitments(): it holds no device table and verifies without this key."""
+        f, s = self.commitments()
+        return VerifyingKey(self.srs, self.keydata, f, s)
 
     def close(self):
         if getattr(self, "_h", None):
             self.ctx._lib.tb_pk_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _verify_batch(ctx, fn, h, instance, instance_len, proofs):
+    B = len(proofs)
+    plen = len(proofs[0])
+    assert all(len(p) == plen for p in proofs)
+    buf = np.frombuffer(b"".join(proofs), np.uint8).copy()
+    inst = _u8(instance)
+    lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+    ok = np.zeros(B, np.uint8)
+    ctx._check(getattr(ctx._lib, fn)(ctx._h, h, B, _ptr(inst), _ptr(lens), _ptr(buf), plen, plen, _ptr(ok)))
+    return [bool(v) for v in ok]
+
+
+class VerifyingKey:
+    """The verifying key of one circuit (tb_vk): halo2's VerifyingKey<vesta::Affine> as Proof::verify uses it
+    (proof.rs:45-54).  Holds the circuit's shape and the fixed / sigma commitments in host memory; refers to `srs`."""
+
+    def __init__(self, srs, keydata, fixed, sigma):
+        self.srs, self.ctx = srs, srs.ctx
+        cs = keydata.cs
+        f, s = _u8(fixed).reshape(-1, 64), _u8(sigma).reshape(-1, 64)
+        assert f.shape[0] == cs.num_fixed and s.shape[0] == len(cs.perm_columns)
+        f, s = np.ascontiguousarray(f), np.ascontiguousarray(s)
+        h = _vp()
+        self.ctx._check(self.ctx._lib.tb_vk_load(self.ctx._h, srs._h, ctypes.byref(keydata.desc), _ptr(f) if f.size else None,
+                                                 _ptr(s) if s.size else None, ctypes.byref(h)))
+        self._h = h
+        self.proof_len = int(self.ctx._lib.tb_vk_proof_len(h))
+
+    def verify_batch(self, instance, instance_len, proofs, ctx=None):
+        """Proof::verify for a batch: proofs = list of byte strings; returns a list of booleans."""
+        return _verify_batch(ctx or self.ctx, "tb_verify_batch_vk", self._h, instance, instance_len, proofs)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self.ctx._lib.tb_vk_free(self._h)
             self._h = None
 
     def __del__(self):
