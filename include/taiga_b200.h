@@ -142,6 +142,34 @@ tb_status tb_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const 
                          const uint32_t* instance_len, const uint8_t seed[32], uint32_t first_proof_index, uint8_t* proofs_out,
                          size_t proof_stride);
 
+/* ---- witness check: MockProver::run(k, circuit, instance).verify() for n_proofs witnesses of one circuit, without proving
+ * (the check of transparent execution, verify_transparently; taiga_halo2/src/circuit/resource_logic_circuit.rs).
+ *   advice, instance, instance_len : as in tb_prove_batch (advice may be a host or a device pointer); advice rows >= usable
+ *                  (the last blinding_factors + 1) are overwritten with pseudorandom values derived from (seed, i), i = the
+ *                  proof's position in the batch: they stand in for MockProver's poisoned cells, so a gate that reads one
+ *                  on an enabled row fails
+ *   seed         : 32 bytes that must be unpredictable to whoever wrote the witnesses (gates are tested through a random
+ *                  fold with y and lookups through a random compression with theta, both drawn from the seed per proof: a
+ *                  failing gate row or lookup input goes unreported with probability at most about
+ *                  (constraints + lookup width) / p, p ~ 2^254, per row; copies are compared exactly)
+ *   counts_out   : n_proofs x 3: rows < usable with a failing constraint, lookup inputs missing from their table, copy cells
+ *                  that differ from their sigma-successor.  A witness passes iff all three are 0.
+ *   failures_out : n_proofs x max_failures records (may be NULL when max_failures = 0): the first max_failures failures of
+ *                  proof i, gates by (row, constraint), then lookups by (lookup, row), then copies by (column, row); unused
+ *                  records are zero.
+ *     TB_FAIL_GATE   constraint `index` (position in constraint_roots) is not zero on row `row`
+ *     TB_FAIL_LOOKUP the input of lookup `index` on row `row` is not among that lookup's table rows < usable
+ *     TB_FAIL_COPY   the cell at permutation-column position `index`, row `row`, differs from its sigma-successor
+ *                    (`other_column`, `other_row`)
+ * A proof's result does not depend on the other witnesses of the batch.  TB_ERR_INVALID covers InstanceTooLarge and a key
+ * whose sigma names a value that is no cell; the context stays usable.  The first check on a key builds its sigma-successor
+ * map (4 bytes per permutation cell, kept on the device); keys that only prove never build it. */
+enum { TB_FAIL_GATE = 1, TB_FAIL_LOOKUP = 2, TB_FAIL_COPY = 3 };
+typedef struct { uint32_t kind, index, row, other_column, other_row; } tb_failure;
+tb_status tb_check_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* advice, const uint8_t* instance,
+                         const uint32_t* instance_len, const uint8_t seed[32], uint32_t max_failures, uint64_t* counts_out,
+                         tb_failure* failures_out);
+
 /* Batched verifier, the counterpart of Proof::verify (taiga_halo2/src/proof.rs:45-54; plonk::verify_proof with
  * SingleVerifier) for n_proofs proofs of one circuit: the transcript is replayed on the host, the final IPA check
  * (one fixed-base MSM over the SRS + one ~100-term MSM per proof) runs on the device.  ok_out[i] = 1 iff proof i is

@@ -203,6 +203,23 @@ struct AdviceTable {
   const uint8_t* data;   // host or device pointer
 };
 
+// One failure MockProver::verify() would report (halo2's VerifyFailure): a constraint not zero on a row (Gate), a lookup input
+// missing from its table (Lookup), or a copied cell that differs from its successor in the permutation (Permutation).
+struct VerifyFailure {
+  enum Kind { Gate = TB_FAIL_GATE, Lookup = TB_FAIL_LOOKUP, Permutation = TB_FAIL_COPY };
+  Kind kind;
+  uint32_t index;        // constraint (position in constraint_roots), lookup, or permutation column position
+  uint32_t row;
+  uint32_t other_column, other_row;   // Permutation: the cell's successor
+};
+// The outcome of checking one witness: the exact counts (rows with a failing constraint, failing lookup inputs, failing copy
+// cells) and the first failures in MockProver's order.  passed() iff all counts are 0.
+struct CheckResult {
+  uint64_t gate_rows = 0, lookup_inputs = 0, copy_cells = 0;
+  std::vector<VerifyFailure> failures;
+  bool passed() const { return gate_rows == 0 && lookup_inputs == 0 && copy_cells == 0; }
+};
+
 // `Proof(Vec<u8>)`, proof.rs:19-22
 class Proof {
  public:
@@ -237,6 +254,32 @@ class Proof {
     ctx.check(tb_prove_batch(ctx.get(), pk.get(), n, circuits[0].data, inst.data(), lens.data(), rng_seed.data(), first_proof_index, buf.data(), plen));
     std::vector<Proof> out;
     for (uint32_t i = 0; i < n; ++i) out.emplace_back(std::vector<uint8_t>(buf.begin() + i * plen, buf.begin() + (i + 1) * plen));
+    return out;
+  }
+
+  // MockProver::run(k, circuit, instance).verify() for n witnesses, without proving (verify_transparently).  `circuits` and
+  // `instances` as in create_batch.  `seed` must be unpredictable to whoever wrote the witnesses: gates and lookups are tested
+  // through random combinations drawn from it (a failure escapes with probability about (constraints + lookup width) / p).
+  static std::vector<CheckResult> check_batch(const ProvingKey& pk, const Params& params, const AdviceTable* circuits, uint32_t n,
+                                              const std::vector<std::vector<std::vector<FieldBytes>>>& instances,
+                                              const std::array<uint8_t, 32>& seed, uint32_t max_failures = 16) {
+    if (&pk.params() != &params) throw Error(TB_ERR_INVALID, "proving key was built for different Params");
+    if (n == 0 || instances.size() != n) throw Error(TB_ERR_INVALID, "one instance per witness is required");
+    std::vector<uint32_t> lens;
+    std::vector<uint8_t> inst = flatten(instances, pk.num_instance(), lens);
+    std::vector<uint64_t> counts(3 * (size_t)n);
+    std::vector<tb_failure> recs((size_t)n * max_failures);
+    const Context& ctx = params.context();
+    ctx.check(tb_check_batch(ctx.get(), pk.get(), n, circuits[0].data, inst.data(), lens.data(), seed.data(), max_failures, counts.data(),
+                             max_failures ? recs.data() : nullptr));
+    std::vector<CheckResult> out(n);
+    for (uint32_t i = 0; i < n; ++i) {
+      out[i].gate_rows = counts[3 * i]; out[i].lookup_inputs = counts[3 * i + 1]; out[i].copy_cells = counts[3 * i + 2];
+      for (uint32_t j = 0; j < max_failures; ++j) {
+        const tb_failure& f = recs[(size_t)i * max_failures + j];
+        if (f.kind) out[i].failures.push_back(VerifyFailure{static_cast<VerifyFailure::Kind>(f.kind), f.index, f.row, f.other_column, f.other_row});
+      }
+    }
     return out;
   }
 

@@ -284,6 +284,13 @@ def satisfied(kd, asg, blinding_seed=0):
     """halo2 MockProver restated: None if `asg` satisfies kd's constraint system, else a message naming the first failure.
     Fixed values and the permutation are the key's (kd.fixed, kd.sigma), advice and instance values the assignment's.
     Advice cells of the blinding rows hold random values, so a gate that reads one on an enabled row fails."""
+    return next(failures(kd, asg, blinding_seed), None)
+
+
+def failures(kd, asg, blinding_seed=0):
+    """Every failure of `asg`, as satisfied's messages, in the order tb_check_batch reports them: gates by (row, constraint),
+    then lookups by (lookup, row), then copies by (permutation column, row).  An instance column longer than the usable rows
+    is reported alone, and a sigma value that is no cell ends the list."""
     cs, n = kd.cs, kd.n
     usable = n - (cs.blinding_factors() + 1)
     br = random.Random(blinding_seed)
@@ -292,7 +299,8 @@ def satisfied(kd, asg, blinding_seed=0):
     instance = [[col[row] if row < len(col) else 0 for row in range(n)] for col in asg.instance]
     for c, col in enumerate(asg.instance):
         if len(col) > usable:
-            return "instance column %d has %d values, more than the %d usable rows" % (c, len(col), usable)
+            yield "instance column %d has %d values, more than the %d usable rows" % (c, len(col), usable)
+            return
 
     def evaluate(node, row, memo):
         if node in memo:
@@ -319,7 +327,7 @@ def satisfied(kd, asg, blinding_seed=0):
         for name, polys in cs.gates:
             for i, p in enumerate(polys):
                 if evaluate(p.node, row, memo):
-                    return "gate %s poly %d is not zero on row %d" % (name, i, row)
+                    yield "gate %s poly %d is not zero on row %d" % (name, i, row)
     for l, lk in enumerate(cs.lookups):
         table = set()
         rows = []
@@ -329,7 +337,7 @@ def satisfied(kd, asg, blinding_seed=0):
             rows.append(tuple(evaluate(i.node, row, memo) for i, _ in lk))
         for row, tup in enumerate(rows):
             if tup not in table:
-                return "lookup %d: input on row %d is not in the table" % (l, row)
+                yield "lookup %d: input on row %d is not in the table" % (l, row)
     # the permutation the key commits to: sigma[i][j] = delta^i' omega^j' names the next cell of (i, j)'s cycle
     cols = cs.perm_columns
     omega = pow(ROOT, 1 << (32 - kd.k), P)
@@ -346,11 +354,11 @@ def satisfied(kd, asg, blinding_seed=0):
         for j in range(usable):
             s = int.from_bytes(kd.sigma[i, j].tobytes(), "little")
             if s not in where:
-                return "sigma of column %d row %d is not a cell" % (i, j)
+                yield "sigma of column %d row %d is not a cell" % (i, j)
+                return
             pi, pj = where[s]
             if grid[c.kind][c.index][j] != grid[cols[pi].kind][cols[pi].index][pj]:
-                return "copy (%r, %d) -> (%r, %d) joins different values" % (c, j, cols[pi], pj)
-    return None
+                yield "copy (%r, %d) -> (%r, %d) joins different values" % (c, j, cols[pi], pj)
 
 
 # ---------------------------------------------------------------- shape summary

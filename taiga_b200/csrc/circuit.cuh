@@ -55,12 +55,17 @@ struct Circuit : Shape {
   mutable std::mutex mu;                                                   // guards the two caches below
   mutable std::map<std::pair<const Ctx*, int>, std::unique_ptr<ProveWs>> ws;
   mutable std::vector<Aff<Fq>> vk_fixed, vk_sigma;   // verifying-key commitments (Montgomery, host), filled on first verification
+  // what tb_check_batch adds, built on its first call (check.cu): the sigma-successor of every permutation cell as a cell index
+  // q * n + r ([P][n]), and the one-constraint programs of plan.single concatenated, with (offset, instructions) per constraint
+  mutable DevMem<uint32_t> sig_next;
+  mutable DevMem<QInstr> single_code; mutable DevMem<int2> single_table; mutable int single_nregs = 0; mutable bool check_ready = false;
   explicit Circuit(Shape&& s) : Shape(std::move(s)) {}
   // the workspace of (context, batch size), marked busy; nullptr if a call is already using it.  Claiming under the lock
-  // lets release_idle() free every workspace that is not marked.
-  ProveWs* claim_workspace(const Ctx* c, int B) const {
+  // lets release_idle() free every workspace that is not marked.  Checks (`check`) keep workspaces apart from proofs: their
+  // buffers differ, and sharing would reallocate on every switch between the two.
+  ProveWs* claim_workspace(const Ctx* c, int B, bool check = false) const {
     std::lock_guard<std::mutex> lk(mu);
-    auto& slot = ws[std::make_pair(c, B)];
+    auto& slot = ws[std::make_pair(c, check ? -B : B)];
     if (!slot) slot.reset(new ProveWs());
     return slot->busy.exchange(1) == 0 ? slot.get() : nullptr;
   }
@@ -80,6 +85,37 @@ struct Circuit : Shape {
     TB_CUDA(cudaMemPoolTrimTo(pool, 0));
   }
 };
+
+// Persistent per-(circuit, batch size) device workspace: the same sequence of requests returns the same pointers on every
+// call, so item tables / scalar programs that embed them are uploaded once and no allocation or host sync happens later.
+template <class T> struct WBuf {
+  T* p = nullptr; size_t n = 0; Ctx* ctx = nullptr;
+  T* get() const { return p; }
+  void zero() { TB_CUDA(cudaMemsetAsync(p, 0, n * sizeof(T), ctx->stream)); }
+};
+struct WsAlloc {
+  Ctx* ctx; const Circuit& C; std::vector<DevMem<uint8_t>>& blocks; size_t cur = 0;
+  template <class T> WBuf<T> buf(size_t count) {
+    size_t bytes = std::max<size_t>(1, count) * sizeof(T);
+    if (cur == blocks.size()) blocks.emplace_back();
+    if (blocks[cur].size() < bytes) {   // try_alloc frees the smaller block first
+      cudaError_t e = blocks[cur].try_alloc(bytes);
+      if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); C.release_idle(ctx->device); e = blocks[cur].try_alloc(bytes); }
+      TB_CUDA(e);
+    }
+    WBuf<T> w; w.p = reinterpret_cast<T*>(blocks[cur].get()); w.n = count; w.ctx = ctx; ++cur;
+    return w;
+  }
+};
+
+
+// The witness of B proofs on the device in Montgomery form (Lagrange basis), shared by the prover and the check:
+// instance columns [B][ni][n] zero past instance_len, advice [B][na][n] (host or device pointer) whose rows >= usable are
+// overwritten with PRF(seed, proof0 + b, rows_tag, c * (bf + 1) + r - usable).  Refuses an instance column longer than the
+// usable rows (InstanceTooLarge); witness_instance_total checks that alone and returns sum(instance_len).
+size_t witness_instance_total(const Circuit& C, const uint32_t* instance_len);
+void upload_witness(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,
+                    const uint8_t* seed, uint32_t proof0, uint32_t rows_tag, Fp* inst_vals, Fp* adv_vals);
 
 // tb_vk: what Proof::verify needs of a circuit.  The commitments are Montgomery affine points, the identity (0, 0).
 struct VerifyingKey {

@@ -263,6 +263,7 @@ struct GatePlan {
   uint32_t num_constraints = 0, t_pl = 0; bool split = false;   // t_pl: permutation + lookup terms folded after the gates
   size_t num_lo = 0; int lo_instr = 0, all_instr = 0;   // what decided the split: low-degree constraints, instructions of them / of all
   std::vector<GateProgram> gate_parts[2], gate_parts_lo[2]; GateProgram lookups;
+  std::vector<GateProgram> single;   // constraint j alone (its value at a row, for naming the constraints a witness breaks there)
 };
 // Degree split: a constraint of degree <= R / 2 is a polynomial of fewer than (R / 2) * n coefficients, so the sum of all such
 // constraints is fixed by its values on every second sub-coset; only the high-degree constraints (and the permutation /
@@ -283,6 +284,11 @@ inline GatePlan gate_plan(const tb_cs_desc* cs, int R, bool allow_split) {
     if (g.split) q_compile_gates_split(cs, lo, GatePlan::nparts[big], &g.gate_parts_lo[big]);
   }
   q_compile_lookups(cs, &g.lookups);
+  for (uint32_t j = 0; j < cs->num_constraints; ++j) {
+    std::vector<GateProgram> one;
+    q_compile_gates_split(cs, {j}, 1, &one);
+    g.single.push_back(std::move(one[0]));
+  }
   return g;
 }
 

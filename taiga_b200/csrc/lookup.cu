@@ -80,23 +80,6 @@ void sort_keys(Ctx* c, Fp* keys, int n, int arrays) {
 }
 
 // ---------------------------------------------------------------- arrangement of the permuted table column
-constexpr int LP_THREADS = 1024;
-__device__ int block_excl_scan(int v, int* sm, int* total) {  // sm: LP_THREADS ints
-  int t = threadIdx.x;
-  sm[t] = v;
-  __syncthreads();
-  for (int d = 1; d < LP_THREADS; d <<= 1) {
-    int x = (t >= d) ? sm[t - d] : 0;
-    __syncthreads();
-    sm[t] += x;
-    __syncthreads();
-  }
-  int incl = sm[t];
-  *total = sm[LP_THREADS - 1];
-  __syncthreads();
-  return incl - v;
-}
-
 // one CTA per (proof, lookup).  A: sorted inputs (canonical, `usable` valid); T: sorted table (canonical).
 // Writes S' (canonical) for rows < usable; scratch `left` holds the unused table values by rank.
 __global__ void __launch_bounds__(LP_THREADS) lookup_arrange_kernel(const Fp* __restrict__ A_all, const Fp* __restrict__ T_all, Fp* __restrict__ left_all,

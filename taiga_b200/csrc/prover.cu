@@ -142,27 +142,33 @@ struct Prog {
   std::vector<ScalarInstr> ins;
   void op(int o, int dst, int a = 0, int b = 0, uint32_t imm = 0) { ScalarInstr i; i.op = (uint16_t)o; i.dst = (uint16_t)dst; i.a = (uint16_t)a; i.b = (uint16_t)b; i.imm = imm; ins.push_back(i); }
 };
-// Persistent per-(circuit, batch size) device workspace: the same sequence of requests returns the same pointers on every
-// call, so item tables / scalar programs that embed them are uploaded once and no allocation or host sync happens later.
-template <class T> struct WBuf {
-  T* p = nullptr; size_t n = 0; Ctx* ctx = nullptr;
-  T* get() const { return p; }
-  void zero() { TB_CUDA(cudaMemsetAsync(p, 0, n * sizeof(T), ctx->stream)); }
-};
-struct WsAlloc {
-  Ctx* ctx; const Circuit& C; std::vector<DevMem<uint8_t>>& blocks; size_t cur = 0;
-  template <class T> WBuf<T> buf(size_t count) {
-    size_t bytes = std::max<size_t>(1, count) * sizeof(T);
-    if (cur == blocks.size()) blocks.emplace_back();
-    if (blocks[cur].size() < bytes) {   // try_alloc frees the smaller block first
-      cudaError_t e = blocks[cur].try_alloc(bytes);
-      if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); C.release_idle(ctx->device); e = blocks[cur].try_alloc(bytes); }
-      TB_CUDA(e);
+size_t witness_instance_total(const Circuit& C, const uint32_t* instance_len) {
+  size_t total = 0;
+  for (uint32_t c = 0; c < C.ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); total += instance_len[c]; }
+  return total;
+}
+
+void upload_witness(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,
+                    const uint8_t* seed, uint32_t proof0, uint32_t rows_tag, Fp* inst_vals, Fp* adv_vals) {
+  const size_t n = C.n, inst_total = witness_instance_total(C, instance_len);
+  const int na = C.na, ni = C.ni, bf = C.bf;
+  cudaStream_t st = ctx->stream;
+  if (ni) {
+    TB_CUDA(cudaMemsetAsync(inst_vals, 0, (size_t)B * ni * n * sizeof(Fp), st));
+    size_t off = 0;
+    for (int c = 0; c < ni; ++c) {
+      if (instance_len[c])
+        TB_CUDA(cudaMemcpy2DAsync(inst_vals + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, B,
+                                  cudaMemcpyHostToDevice, st));
+      off += instance_len[c];
     }
-    WBuf<T> w; w.p = reinterpret_cast<T*>(blocks[cur].get()); w.n = count; w.ctx = ctx; ++cur;
-    return w;
+    fe_to_mont<Fp>(ctx, inst_vals, (size_t)B * ni * n);
   }
-};
+  TB_CUDA(cudaMemcpyAsync(adv_vals, advice, (size_t)B * na * n * 32, cudaMemcpyDefault, st));  // host or device pointer
+  fe_to_mont<Fp>(ctx, adv_vals, (size_t)B * na * n);
+  for (int c = 0; c < na; ++c)
+    prf_fill(ctx, seed, proof0, rows_tag, (uint32_t)(c * (bf + 1)), adv_vals + (size_t)c * n + C.usable, (long long)na * n, 1, bf + 1, B);
+}
 
 static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice_host, const uint8_t* instance_host, const uint32_t* instance_len,
                         const uint8_t* seed, uint32_t proof0, uint8_t* proofs_out, size_t proof_stride) {
@@ -175,8 +181,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   const int O_ADV = 0, O_INST = na, O_PZ = na + ni, O_LZ = na + ni + nsets, O_LPIN = O_LZ + L, O_LPTAB = O_LZ + 2 * L;
   const long long PS = (long long)NC * nn;   // per-proof stride of the merged buffers
   cudaStream_t st = ctx->stream;
-  size_t inst_total = 0;
-  for (int c = 0; c < ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); inst_total += instance_len[c]; }
+  witness_instance_total(C, instance_len);
   ProveWs* claimed = C.claim_workspace(ctx, B);
   TB_REQUIRE(claimed != nullptr, "this proving key / context / batch size is already proving on another thread (a tb_ctx is bound to one thread)");
   ProveWs& pws = *claimed;
@@ -244,24 +249,10 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   WBuf<Fp> inst_vals; inst_vals.p = first.get(); inst_vals.n = (size_t)B * ni * n; inst_vals.ctx = ctx;
   WBuf<Fp> adv_vals; adv_vals.p = first.get() + (size_t)B * ni * n; adv_vals.n = (size_t)B * na * n; adv_vals.ctx = ctx;
   Fp* const inst_polys = polys.get() + (size_t)O_INST * n;
-  if (ni) inst_vals.zero();
-  if (ni) {
-    size_t off = 0;
-    for (int c = 0; c < ni; ++c) {
-      if (instance_len[c])
-        TB_CUDA(cudaMemcpy2DAsync(inst_vals.get() + (size_t)c * n, (size_t)ni * n * 32, instance_host + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, B,
-                                  cudaMemcpyHostToDevice, st));
-      off += instance_len[c];
-    }
-    fe_to_mont<Fp>(ctx, inst_vals.get(), (size_t)B * ni * n);
-    launch(ctx, fill_const_kernel, (B * ni + 63) / 64, 64, 0, blinds.get(), (size_t)B * ni, Fp::one());
-  }
-  // ---- advice columns: upload, blinding rows, commit, iNTT
   Fp* const adv_polys = polys.get() + (size_t)O_ADV * n;
-  TB_CUDA(cudaMemcpyAsync(adv_vals.get(), advice_host, (size_t)B * na * n * 32, cudaMemcpyDefault, st));  // host or device pointer
-  fe_to_mont<Fp>(ctx, adv_vals.get(), (size_t)B * na * n);
-  for (int c = 0; c < na; ++c)
-    prf_fill(ctx, seed, proof0, R_ADVICE_ROWS, (uint32_t)(c * (bf + 1)), adv_vals.get() + (size_t)c * n + C.usable, (long long)na * nn, 1, bf + 1, B);
+  upload_witness(ctx, C, B, advice_host, instance_host, instance_len, seed, proof0, R_ADVICE_ROWS, inst_vals.get(), adv_vals.get());
+  if (ni) launch(ctx, fill_const_kernel, (B * ni + 63) / 64, 64, 0, blinds.get(), (size_t)B * ni, Fp::one());
+  // ---- advice columns: commit, iNTT
   prf_fill(ctx, seed, proof0, R_ADVICE_BLIND, 0, VP(V_ADV_BLIND), NV, 1, na, B);
   poly_copy(ctx, blinds.get() + (size_t)B * ni, na, VP(V_ADV_BLIND), NV, na, B);
   srs.commit(ctx, true, first.get(), nn, B * (ni + na), blinds.get(), pts.get());   // [B*ni instance | B*na advice]

@@ -24,7 +24,9 @@ struct Transcripts {
 };
 // blinding PRF tags (must match oracle/plonk.cpp RndTag)
 enum RndTag { R_ADVICE_ROWS = 1, R_ADVICE_BLIND, R_LK_IN_ROWS, R_LK_TAB_ROWS, R_LK_IN_BLIND, R_LK_TAB_BLIND, R_PERM_ROWS, R_PERM_BLIND,
-              R_LKZ_ROWS, R_LKZ_BLIND, R_RANDOM_POLY, R_RANDOM_BLIND, R_H_BLIND, R_QPRIME_BLIND, R_S_POLY, R_S_BLIND, R_IPA_L, R_IPA_R };
+              R_LKZ_ROWS, R_LKZ_BLIND, R_RANDOM_POLY, R_RANDOM_BLIND, R_H_BLIND, R_QPRIME_BLIND, R_S_POLY, R_S_BLIND, R_IPA_L, R_IPA_R,
+              // tb_check_batch's: the advice blinding rows, the gate fold y and the lookup compression theta (no proof uses these)
+              R_CHECK_ROWS = 64, R_CHECK_Y, R_CHECK_THETA };
 void prf_fill(Ctx* c, const uint8_t* seed32, uint32_t proof0, uint32_t tag, uint32_t idx0, Fp* out, long long stride, long long elem_stride,
               int count, int B);
 

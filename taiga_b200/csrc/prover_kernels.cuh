@@ -10,6 +10,26 @@ namespace tb {
 void lookup_keys(Ctx* c, Fp* keys, const Fp* vals, int n, int usable, int arrays);      // Montgomery -> canonical sort keys (+ sentinels)
 void sort_keys(Ctx* c, Fp* keys, int n, int arrays);                                      // ascending, canonical-integer order
 void lookup_arrange(Ctx* c, const Fp* sortedA, const Fp* sortedT, Fp* scratch, Fp* S, int n, int usable, int arrays, uint32_t* d_err);
+#ifdef __CUDACC__
+// exclusive prefix sum of one int per thread over a CTA of LP_THREADS threads (lookup_arrange, the check's report)
+constexpr int LP_THREADS = 1024;
+__device__ inline int block_excl_scan(int v, int* sm, int* total) {  // sm: LP_THREADS ints
+  int t = threadIdx.x;
+  sm[t] = v;
+  __syncthreads();
+  for (int d = 1; d < LP_THREADS; d <<= 1) {
+    int x = (t >= d) ? sm[t - d] : 0;
+    __syncthreads();
+    sm[t] += x;
+    __syncthreads();
+  }
+  int incl = sm[t];
+  *total = sm[LP_THREADS - 1];
+  __syncthreads();
+  return incl - v;
+}
+
+#endif
 
 // ---------------------------------------------------------------- quotient.cu
 // Row-parallel interpreter of the programs of gates.cuh.  Temporaries live in a shared-memory register file laid out
@@ -33,6 +53,10 @@ struct QData {
 };
 void q_run(Ctx* c, const QProgram& prog, const QData& d, int B);
 void q_run_parts(Ctx* c, const std::vector<QProgram>& progs, QData d, long long part_stride, int B);
+// One program per constraint on a short list of rows: nonzero[b][s][j] = (program j on row rows[b * M + s] != 0) for
+// s < min(M, nrows[b]).  code / table: the programs concatenated, (offset, instructions) of each; nregs: the largest.
+void q_run_rows(Ctx* c, const QInstr* code, const int2* table, int nprogs, int nregs, const QData& d, const uint32_t* rows, const uint64_t* nrows,
+                long long nrows_stride, int M, uint8_t* nonzero, int B);
 
 // permutation + lookup terms of the quotient, folded onto the gate accumulator, times 1/(X^n - 1) (constant per sub-coset)
 struct QFinish {

@@ -56,6 +56,21 @@ __global__ void __launch_bounds__(128) q_interp_kernel(const __grid_constant__ Q
   if (d.gate_out) st_fe(d.gate_out + (long long)blockIdx.z * pl.part_stride + (long long)b * d.gate_pstride + row, m.get(m.slot(nregs)));
 }
 
+// The same interpreter on listed rows: thread (s, b) of program blockIdx.z evaluates row rows[b * M + s], s < min(M, nrows[b])
+__global__ void __launch_bounds__(128) q_interp_rows_kernel(const QInstr* __restrict__ code, const int2* __restrict__ table, int nregs, QData d,
+                                                            const uint32_t* __restrict__ rows, const uint64_t* __restrict__ nrows, long long nrows_stride, int M,
+                                                            uint8_t* __restrict__ nonzero) {
+  extern __shared__ uint4 q_smem[];
+  const int T = blockDim.x, tid = threadIdx.x, s = blockIdx.x * T + tid, b = blockIdx.y, j = blockIdx.z;
+  if ((uint64_t)s >= min((uint64_t)M, nrows[(long long)b * nrows_stride])) return;
+  const int2 e = table[j];
+  const int row = (int)rows[(size_t)b * M + s];
+  QRowMachine m = {reinterpret_cast<const uint4*>(code + e.x), q_smem + tid, q_smem + (size_t)(nregs + 2) * T + tid, T, row, b,
+                   d.adv + (long long)b * d.adv_pstride, d.inst + (long long)b * d.inst_pstride, d.chal + (long long)b * d.chal_stride, d};
+  gate_interp(m, nregs, e.y);
+  nonzero[((size_t)b * M + s) * gridDim.z + j] = m.get(m.slot(nregs)).is_zero() ? 0 : 1;
+}
+
 static double program_muls(const QProgram& p) {   // field multiplications per evaluated row
   double m = 0;
   for (const QInstr& in : p.prog.code) { const int op = in.w0 & 0xff; m += (op == Q_MUL || op == Q_FOLD_Y || op == Q_FOLD_A || op == Q_FOLD_S || op == Q_GFOLD) ? 1.0 : op == Q_GEND ? 2.0 : 0.0; }
@@ -85,6 +100,17 @@ void q_run_parts(Ctx* c, const std::vector<QProgram>& progs, QData d, long long 
   for (int p = 0; p < pl.nparts; ++p) c->work[PC_QUOT_GATES] += program_muls(progs[p]) * (double)d.n * B;
   for (int p = 0; p < pl.nparts; ++p) { pl.prog[p] = progs[p].dev.get(); pl.ninstr[p] = (int)progs[p].prog.code.size(); nregs = nregs > progs[p].prog.nregs ? nregs : progs[p].prog.nregs; }
   q_launch(c, pl, nregs, d, B);
+}
+void q_run_rows(Ctx* c, const QInstr* code, const int2* table, int nprogs, int nregs, const QData& d, const uint32_t* rows, const uint64_t* nrows,
+                long long nrows_stride, int M, uint8_t* nonzero, int B) {
+  if (M == 0 || nprogs == 0) return;
+  ProfScope prof_scope(c, PC_QUOT_GATES);
+  c->opt_in_smem(q_interp_rows_kernel, 96 * 1024);
+  int T = (96 * 1024) / ((nregs + 2) * 32);   // as q_launch: the register file fits 96 KiB
+  T = T >= 128 ? 128 : (T / 16) * 16;
+  while (T > 32 && T / 2 >= M) T >>= 1;        // few listed rows: small CTAs
+  const size_t smem = (size_t)(nregs + 2) * T * 32;
+  launch(c, q_interp_rows_kernel, dim3((M + T - 1) / T, B, nprogs), T, smem, code, table, nregs, d, rows, nrows, nrows_stride, M, nonzero);
 }
 
 }  // namespace tb

@@ -3,6 +3,7 @@
 The product path has no CPU fallback: if the CUDA library is missing or no sm_90 device is usable this
 module raises instead of computing anything on the host.
 """
+import collections
 import ctypes
 import os
 
@@ -62,7 +63,28 @@ _SIGS = {
     "tb_vk_free": (None, [_vp]),
     "tb_vk_proof_len": (_sz, [_vp]),
     "tb_verify_batch_vk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
+    "tb_check_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp]),
 }
+
+TB_FAIL_GATE, TB_FAIL_LOOKUP, TB_FAIL_COPY = 1, 2, 3
+# one record of tb_check_batch (tb_failure): kind TB_FAIL_*; gate: constraint `index` on `row`; lookup: lookup `index`, input row
+# `row`; copy: permutation column position `index`, `row`, and its sigma-successor (other_column, other_row)
+Failure = collections.namedtuple("Failure", "kind index row other_column other_row")
+
+
+def render_failure(keydata, f):
+    """The message circuits_random.satisfied gives for failure `f` of a witness of `keydata`'s circuit."""
+    cs = keydata.cs
+    if f.kind == TB_FAIL_GATE:
+        names = [(name, i) for name, polys in cs.gates for i in range(len(polys))]
+        name, i = names[f.index]
+        return "gate %s poly %d is not zero on row %d" % (name, i, f.row)
+    if f.kind == TB_FAIL_LOOKUP:
+        return "lookup %d: input on row %d is not in the table" % (f.index, f.row)
+    if f.kind == TB_FAIL_COPY:
+        cols = cs.perm_columns
+        return "copy (%r, %d) -> (%r, %d) joins different values" % (cols[f.index], f.row, cols[f.other_column], f.other_row)
+    raise ValueError("unknown failure kind %d" % f.kind)
 
 
 def exported_symbols():
@@ -288,6 +310,38 @@ class ProvingKey:
     def verify_batch(self, instance, instance_len, proofs, ctx=None):
         """Proof::verify for a batch: proofs = list of byte strings; returns a list of booleans."""
         return _verify_batch(ctx or self.ctx, "tb_verify_batch", self._h, instance, instance_len, proofs)
+
+    def check_batch(self, advice, instance, instance_len, seed, max_failures=16, ctx=None):
+        """MockProver::run(k, circuit, instance).verify() for a batch, without proving: advice / instance as in prove_batch
+        (advice may also be a pinned-host or device torch tensor).  `seed` (32 bytes) draws the random fold of the gates and
+        the compression of the lookups; it must be unpredictable to whoever wrote the witnesses.  Returns per witness
+        (counts, failures): counts = (rows with a failing constraint, failing lookup inputs, failing copy cells), failures
+        = the first max_failures Failure records, gates by (row, constraint), then lookups, then copies.  A witness passes
+        iff all counts are 0; render_failure names a record as circuits_random.satisfied does."""
+        ctx = ctx or self.ctx
+        kd = self.keydata
+        per = kd.cs.num_advice * kd.n * 32
+        if hasattr(advice, "data_ptr"):
+            nbytes = advice.numel() * advice.element_size()
+        else:
+            advice = _u8(advice)
+            nbytes = advice.size
+        assert nbytes % per == 0
+        B = nbytes // per
+        inst = _u8(instance)
+        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+        assert inst.size >= B * int(lens.sum()) * 32
+        seed = _u8(np.frombuffer(bytes(seed), np.uint8))
+        assert seed.size == 32
+        counts = np.zeros((B, 3), np.uint64)
+        recs = np.zeros((B, max(1, max_failures), 5), np.uint32)
+        ctx._check(ctx._lib.tb_check_batch(ctx._h, self._h, B, _ptr(advice), _ptr(inst), _ptr(lens), _ptr(seed), max_failures,
+                                           _ptr(counts), _ptr(recs) if max_failures else None))
+        out = []
+        for b in range(B):
+            fails = [Failure(*(int(v) for v in r)) for r in recs[b, :max_failures] if r[0]]   # unused records are zero
+            out.append((tuple(int(c) for c in counts[b]), fails))
+        return out
 
     def verifying_key(self):
         """The VerifyingKey of this circuit, built from commitments(): it holds no device table and verifies without this key."""

@@ -117,6 +117,21 @@ class ProverService:
             out[kind] += results[(kind, lo)]
         return out["c"], out["v"]
 
+    def check_ptx_batch(self, wit, seed, max_failures=16):
+        """The batched verify_transparently: MockProver::run(15, ..).verify() of all 2P Compliance and 4P VP witnesses of
+        `wit` (what synthesize_ptx returns), one check_batch call per circuit.  `seed` (32 bytes) must be unpredictable to
+        whoever wrote the witnesses.  Returns one list per partial transaction of its failing proofs, as
+        (circuit "compliance" | "vp", index of the proof within the partial transaction, counts, [message]); an empty list
+        means every proof of that partial transaction passes."""
+        n_ptx = len(wit["c_inst"]) // COMPLIANCE_PER_PTX
+        out = [[] for _ in range(n_ptx)]
+        for name, pk, adv, inst, lens, per in (("compliance", self.pk_c, wit["c_adv"], wit["c_inst"], wit["c_len"], COMPLIANCE_PER_PTX),
+                                               ("vp", self.pk_v, wit["v_adv"], wit["v_inst"], wit["v_len"], VP_PER_PTX)):
+            for i, (counts, fails) in enumerate(pk.check_batch(adv, inst, lens, seed, max_failures)):
+                if any(counts):
+                    out[i // per].append((name, i % per, counts, [lib.render_failure(pk.keydata, f) for f in fails]))
+        return out
+
     @property
     def launch_count(self):
         return sum(c.launch_count for c in self.contexts)
