@@ -135,7 +135,7 @@ void powers(Ctx* c, Fp* out, long long out_stride, const Fp* x, long long x_stri
 // dependent chain is 8 (local Horner) + 9 (block suffix composition) + <= 7 (cluster composition over distributed shared
 // memory) + 8 (replay with the incoming carry) multiply-adds, spread over 8 SMs -- it used to be 64 + 9 + 64 on one SM.
 // The kernel is pure latency (one polynomial per proof per opening point).  Polynomials shorter than 4096 use a single CTA.
-constexpr int KD_THREADS = 512, KD_CLUSTER = 8, KD_MAX_M = 8;
+// KD_THREADS, KD_CLUSTER, KD_MAX_M and the length limit KD_MAX_N are in prover.cuh.
 __global__ void __launch_bounds__(KD_THREADS) kate_div_kernel(Fp* out, long long out_stride, const Fp* in, long long in_stride, const Fp* zs,
                                                                long long z_stride, int n, int cs /* CTAs per polynomial */) {
   namespace cg = cooperative_groups;
@@ -197,8 +197,8 @@ __global__ void __launch_bounds__(KD_THREADS) kate_div_kernel(Fp* out, long long
 void poly_kate_div(Ctx* c, Fp* out, long long out_stride, const Fp* in, long long in_stride, const Fp* z, long long z_stride, int n, int B) {
   ProfScope prof_scope(c, PC_POLY);
   TB_REQUIRE((n & (n - 1)) == 0, "kate division needs a power-of-two length");
+  TB_REQUIRE(n >= 1 && n <= KD_MAX_N, "kate division: polynomial too long for one cluster");
   const int cs = n >= KD_CLUSTER * KD_THREADS ? KD_CLUSTER : 1;
-  TB_REQUIRE(n / (cs * (n / cs < KD_THREADS ? n / cs : KD_THREADS)) <= KD_MAX_M, "kate division: polynomial too long for one cluster");
   launch_cluster(c, cs, kate_div_kernel, (unsigned)(B * cs), KD_THREADS, 0, out, out_stride, in, in_stride, z, z_stride, n, cs);
 }
 

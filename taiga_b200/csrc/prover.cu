@@ -36,6 +36,8 @@ static Circuit* circuit_load(Ctx* ctx, const Srs* srs, const tb_cs_desc* cs, con
   std::unique_ptr<Circuit> Cp(new Circuit(shape_build(cs, srs->k, tb_tune("TB_Q_SPLIT", 1) != 0)));
   Circuit& C = *Cp;
   C.srs = srs;
+  // refused before any device work: the multiopen would fail only after the rest of every proof had been computed
+  TB_REQUIRE(C.n <= (size_t)KD_MAX_N, "circuit has more rows than the multiopen's Kate division handles: at most " + std::to_string(KD_MAX_N));
   { Fp step = omega_k<Fp>(C.ext_k).pow_u64(C.n);
     std::vector<Fp> wr(C.R); Fp wri = step.inv(); wr[0] = Fp::one(); for (int e = 1; e < C.R; ++e) wr[e] = wr[e - 1] * wri;
     C.wr_inv = DevMem<Fp>(wr); }

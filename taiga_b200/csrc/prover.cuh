@@ -41,7 +41,11 @@ void poly_add_at(Ctx* c, Fp* v, long long stride, int idx, const Fp* s, long lon
 struct EvalItem { const Fp* base; long long bstride; int point; int pad; };
 // evals[b*ev_stride + t] = poly_t(points[b*pt_stride + items[t].point]),  poly_t = items[t].base + b*items[t].bstride, n coefficients
 void poly_eval(Ctx* c, const EvalItem* d_items, int nitems, const Fp* points, long long pt_stride, Fp* evals, long long ev_stride, int n, int B);
-// out[b] = quotient of (in[b](X) - in[b](z_b)) / (X - z_b), zero padded to n coefficients (halo2 kate_division + resize)
+// out[b] = quotient of (in[b](X) - in[b](z_b)) / (X - z_b), zero padded to n coefficients (halo2 kate_division + resize).
+// One cluster of KD_CLUSTER CTAs x KD_THREADS threads x at most KD_MAX_M coefficients per thread divides one polynomial, so
+// n <= KD_MAX_N; tb_circuit_load refuses a circuit with more rows, since its multiopen could not be divided.
+constexpr int KD_THREADS = 512, KD_CLUSTER = 8, KD_MAX_M = 8;
+constexpr int KD_MAX_N = KD_CLUSTER * KD_THREADS * KD_MAX_M;
 void poly_kate_div(Ctx* c, Fp* out, long long out_stride, const Fp* in, long long in_stride, const Fp* z, long long z_stride, int n, int B);
 void batch_inverse(Ctx* c, Fp* v, size_t count);  // elementwise, 0 -> 0
 // out[b][0] = 1, out[b][i] = prod_{j<i} in[b][j]   (count independent vectors of n; n a power of two)

@@ -1,7 +1,8 @@
 """GPU parity on random and boundary constraint systems (taiga_b200/circuits_random.py; the same shapes and seeds the CPU
 file test_random_shapes_oracle.py proves on the oracle).  For every shape the CUDA prover's keygen commitments and proofs
 of two distinct witnesses must equal the oracle's byte for byte; a mismatch is reported by proof section.  Each shape is
-proved once more under one set of tuning knobs, and two shapes beyond the supported envelope must be refused at load."""
+proved once more under one set of tuning knobs, and shapes beyond the supported envelope (three shapes, and a circuit with
+more rows than the Kate division divides) must be refused at load."""
 import numpy as np
 import pytest
 
@@ -108,6 +109,27 @@ def test_shapes_beyond_the_envelope_are_refused(gpu_ctx, oracle_cpu, srs_for, bu
     with pytest.raises(lib.TaigaB200Error) as e:
         gsrs.load_circuit(kd)
     assert e.value.status == lib.TB_ERR_INVALID, str(e.value)
+    adv, inst, lens = kd_ok.witness_arrays(make(4))
+    seed = bytes(range(32))
+    proof = gsrs.load_circuit(kd_ok).prove_batch(adv[None], inst[None], lens, seed, first_proof_index=9)[0]
+    assert proof == oracle_cpu.OracleKey(kd_ok, srs).prove(adv, inst, lens, seed, proof_index=9)
+
+
+def test_circuit_beyond_the_kate_division_is_refused_at_load(gpu_ctx, oracle_cpu, srs_for, srs_fixture):
+    """k = 16: the multiopen's Kate division divides at most 2^15 coefficients, so tb_circuit_load refuses the circuit
+    (TB_ERR_INVALID, naming the limit) instead of tb_prove_batch failing after the rest of the proof.  The refusal comes
+    before the SRS's points are read, so the k = 15 fixture's points, repeated to 2^16, stand in for a k = 16 SRS."""
+    s = srs_fixture
+    g16 = gpu_ctx.load_srs(16, np.concatenate([s["g"], s["g"]]), np.concatenate([s["g_lagrange"], s["g_lagrange"]]), s["w"], s["u"])
+    try:
+        with pytest.raises(lib.TaigaB200Error) as e:
+            g16.load_circuit(_rotation(16, 1))
+        assert e.value.status == lib.TB_ERR_INVALID, str(e.value)
+        assert "Kate division" in str(e.value) and str(1 << 15) in str(e.value), str(e.value)
+    finally:
+        g16.close()
+    kd_ok, make = cr.boundary("deg4")
+    srs, gsrs = srs_for(kd_ok.k)
     adv, inst, lens = kd_ok.witness_arrays(make(4))
     seed = bytes(range(32))
     proof = gsrs.load_circuit(kd_ok).prove_batch(adv[None], inst[None], lens, seed, first_proof_index=9)[0]
