@@ -195,6 +195,32 @@ size_t tb_vk_proof_len(const tb_vk* vk);
 tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk, uint32_t n_proofs, const uint8_t* instance, const uint32_t* instance_len,
                              const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out);
 
+/* ---- batch verifier: halo2's plonk::BatchVerifier (add_proof, finalize -> bool), one verdict for any number of proofs of any
+ * number of circuits over one SRS (the proofs of a ShieldedPartialTxBundle, shielded_ptx.rs:137-153).
+ *   create    binds the batch to `srs` (which must outlive it) and to the 32-byte `seed`.
+ *   add       takes n_proofs (1..4096) proofs of the circuit of `vk`, with the arguments of tb_verify_batch_vk; call it any
+ *             number of times, with any verifying keys on the batch's SRS.
+ *   finalize  *ok_out = 1 iff every proof added since create would be accepted by tb_verify_batch_vk.  It consumes the batch:
+ *             only free is allowed afterwards.  An empty batch gives 1.
+ * The j-th proof added (j counts from 0 over the batch's lifetime, across calls) gets the weight rho_j = PRF(seed, j), and the
+ * batch accepts iff sum_j rho_j * (final-check sum of proof j) is the identity: one fixed-base MSM over the SRS at finalize,
+ * one variable-base MSM per add.  The seed must be unpredictable to whoever made the proofs: then a batch that contains a proof
+ * failing its own check is accepted with probability at most 1/p (p ~ 2^254).  Draw a fresh seed per batch.
+ * A proof rejected before its final check (a proof_len other than tb_vk_proof_len, an encoding that does not decode, the
+ * identity, a non-canonical scalar or instance value, trailing bytes) makes the verdict 0; add still returns TB_OK.
+ * add refuses (TB_ERR_INVALID) a vk on another SRS, n_proofs of 0 or more than 4096, proof_stride < proof_len, an instance
+ * column longer than the usable rows, more than 2^32 proofs in all, and any call after finalize; a refused add leaves the
+ * batch as it was.  An add that fails part way (TB_ERR_CUDA) leaves the batch good only for free; finalize then refuses it.
+ * Device state: n + 1 field elements and one point, on the SRS's device.  Any context on that device may use the batch, one
+ * thread at a time. */
+typedef struct tb_batch_verifier tb_batch_verifier;
+tb_status tb_batch_verifier_create(tb_ctx* ctx, const tb_srs* srs, const uint8_t seed[32], tb_batch_verifier** out);
+tb_status tb_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv, const tb_vk* vk, uint32_t n_proofs,
+                                const uint8_t* instance, const uint32_t* instance_len,
+                                const uint8_t* proofs, size_t proof_stride, size_t proof_len);
+tb_status tb_batch_verifier_finalize(tb_ctx* ctx, tb_batch_verifier* bv, uint8_t* ok_out);
+void tb_batch_verifier_free(tb_batch_verifier* bv);
+
 #ifdef __cplusplus
 }
 #endif

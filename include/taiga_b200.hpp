@@ -340,6 +340,43 @@ class Proof {
     return out;
   }
   std::vector<uint8_t> bytes_;
+  friend class BatchVerifier;
+};
+
+// plonk::BatchVerifier: proofs of any circuits over one Params, one verdict.  add_proof / add_proofs queue nothing on the host:
+// each call replays its proofs and folds their random-weighted final checks into the batch on the device; finalize() runs
+// the one remaining MSM and returns true iff every proof added would verify on its own.  `seed` draws the weights and must
+// be unpredictable to whoever made the proofs (a batch holding a bad proof is then accepted with probability at most 1/p):
+// draw a fresh one per batch.  finalize() consumes the batch.  Throws Error for a refused call (a key built for other
+// Params, a call after finalize) and for device failures; a proof that does not even decode is not an error, it makes
+// finalize() return false.
+class BatchVerifier {
+ public:
+  BatchVerifier(const Params& params, const std::array<uint8_t, 32>& seed) : params_(&params) {
+    tb_batch_verifier* b = nullptr;
+    params.context().check(tb_batch_verifier_create(params.context().get(), params.get(), seed.data(), &b));
+    bv_.reset(b);
+  }
+  void add_proof(const VerifyingKey& vk, const std::vector<std::vector<FieldBytes>>& instance, const Proof& proof) {
+    add_proofs(vk, {proof}, {instance});
+  }
+  // `instances[i]`: one vector per instance column of proof i; at most 4096 proofs per call
+  void add_proofs(const VerifyingKey& vk, const std::vector<Proof>& proofs, const std::vector<std::vector<std::vector<FieldBytes>>>& instances) {
+    if (&vk.params() != params_) throw Error(TB_ERR_INVALID, "verifying key was built for different Params");
+    Proof::verify_with(*params_, proofs, instances, vk.num_instance(), [&](uint32_t n, const uint8_t* inst, const uint32_t* lens, const uint8_t* buf, size_t plen, uint8_t*) {
+      return tb_batch_verifier_add(params_->context().get(), bv_.get(), vk.get(), n, inst, lens, buf, plen, plen);
+    });
+  }
+  bool finalize() {
+    uint8_t ok = 0;
+    params_->context().check(tb_batch_verifier_finalize(params_->context().get(), bv_.get(), &ok));
+    return ok == 1;
+  }
+
+ private:
+  struct Del { void operator()(tb_batch_verifier* b) const { tb_batch_verifier_free(b); } };
+  const Params* params_;
+  std::unique_ptr<tb_batch_verifier, Del> bv_;
 };
 
 }  // namespace taiga_b200

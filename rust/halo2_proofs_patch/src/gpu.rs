@@ -374,3 +374,59 @@ pub fn verify_batch_gpu(gp: &GpuParams, gpk: &GpuProvingKey, instances: &[&[&[F]
 pub fn verify_batch_gpu_vk(gp: &GpuParams, gvk: &GpuVerifyingKey, instances: &[&[&[F]]], proofs: &[&[u8]]) -> Result<Vec<bool>, Error> {
     verify_with(gp, instances, proofs, |ctx, n, inst, lens, flat, plen, ok| unsafe { tb::tb_verify_batch_vk(ctx, gvk.vk, n, inst, lens, flat, plen, plen, ok) })
 }
+
+/// `plonk::BatchVerifier` on the device (tb_batch_verifier_*; the FFI declarations come from taiga_b200.h through bindgen):
+/// proofs of any circuits over `gp`'s SRS, one verdict.  Each `add_proofs` call replays its proofs and folds their
+/// random-weighted final checks into the batch on the device; `finalize` runs the one remaining MSM.  The weights come from a
+/// seed drawn from `rng` at `new`, which must be unpredictable to whoever made the proofs (then a batch that holds a bad proof is
+/// accepted with probability at most 1/p).  Replaces the serial `verify_proof` loop of ShieldedPartialTxBundle::execute
+/// (transaction.rs:246-257, shielded_ptx.rs:137-153): see INTEGRATION.md.
+pub struct GpuBatchVerifier<'a> {
+    gp: &'a GpuParams,
+    bv: *mut tb::tb_batch_verifier,
+}
+
+impl<'a> GpuBatchVerifier<'a> {
+    pub fn new(gp: &'a GpuParams, mut rng: impl RngCore) -> Result<Self, Error> {
+        let mut seed = [0u8; 32];
+        rng.fill_bytes(&mut seed);
+        let mut bv = std::ptr::null_mut();
+        let ctx = gp.ctx.lock().unwrap();
+        let st = unsafe { tb::tb_batch_verifier_create(*ctx, gp.srs, seed.as_ptr(), &mut bv) };
+        if st != 0 {
+            return Err(map_status(st, *ctx));
+        }
+        Ok(GpuBatchVerifier { gp, bv })
+    }
+
+    /// `add_proof` for each of `proofs` (one circuit, at most 4096 per call).  A proof that does not even decode is not an
+    /// error: it makes `finalize` return false.
+    pub fn add_proofs(&mut self, gvk: &GpuVerifyingKey, instances: &[&[&[F]]], proofs: &[&[u8]]) -> Result<(), Error> {
+        let bv = self.bv;
+        verify_with(self.gp, instances, proofs, |ctx, n, inst, lens, flat, plen, _ok| unsafe {
+            tb::tb_batch_verifier_add(ctx, bv, gvk.vk, n, inst, lens, flat, plen, plen)
+        })
+        .map(|_| ())
+    }
+
+    pub fn add_proof(&mut self, gvk: &GpuVerifyingKey, instance: &[&[F]], proof: &[u8]) -> Result<(), Error> {
+        self.add_proofs(gvk, &[instance], &[proof])
+    }
+
+    /// true iff every proof added would pass `Proof::verify` (halo2's `BatchVerifier::finalize`; an empty batch is true)
+    pub fn finalize(self) -> Result<bool, Error> {
+        let mut ok = 0u8;
+        let ctx = self.gp.ctx.lock().unwrap();
+        let st = unsafe { tb::tb_batch_verifier_finalize(*ctx, self.bv, &mut ok) };
+        if st != 0 {
+            return Err(map_status(st, *ctx));
+        }
+        Ok(ok == 1)
+    }
+}
+
+impl Drop for GpuBatchVerifier<'_> {
+    fn drop(&mut self) {
+        unsafe { tb::tb_batch_verifier_free(self.bv) }
+    }
+}

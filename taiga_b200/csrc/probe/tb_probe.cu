@@ -67,5 +67,9 @@ tb_status tbp_lookup_arrange(tb_ctx* ctx, const void* sorted_a, const void* sort
   lookup_arrange(&ctx->c, CFP(sorted_a), CFP(sorted_t), FP(scratch), FP(s), n, usable, arrays, reinterpret_cast<uint32_t*>(err));
   TB_API_END(ctx)
 }
+// the batch verifier's g-term (verifier.cu): G (2^kk scalars) += the terms of K proofs, us [K][kk], ab [K][2]
+tb_status tbp_batch_g_scalars(tb_ctx* ctx, void* G, const void* us, const void* ab, int kk, int K) {
+  TB_API_BEGIN(ctx) batch_g_scalars(&ctx->c, FP(G), CFP(us), CFP(ab), kk, K); TB_API_END(ctx)
+}
 
 }  // extern "C"

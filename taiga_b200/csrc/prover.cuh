@@ -26,7 +26,9 @@ struct Transcripts {
 enum RndTag { R_ADVICE_ROWS = 1, R_ADVICE_BLIND, R_LK_IN_ROWS, R_LK_TAB_ROWS, R_LK_IN_BLIND, R_LK_TAB_BLIND, R_PERM_ROWS, R_PERM_BLIND,
               R_LKZ_ROWS, R_LKZ_BLIND, R_RANDOM_POLY, R_RANDOM_BLIND, R_H_BLIND, R_QPRIME_BLIND, R_S_POLY, R_S_BLIND, R_IPA_L, R_IPA_R,
               // tb_check_batch's: the advice blinding rows, the gate fold y and the lookup compression theta (no proof uses these)
-              R_CHECK_ROWS = 64, R_CHECK_Y, R_CHECK_THETA };
+              R_CHECK_ROWS = 64, R_CHECK_Y, R_CHECK_THETA,
+              // tb_batch_verifier's weight of the j-th proof of a batch: PRF(seed, j, R_BATCH_WEIGHT, 0) (no proof uses it)
+              R_BATCH_WEIGHT = 80 };
 void prf_fill(Ctx* c, const uint8_t* seed32, uint32_t proof0, uint32_t tag, uint32_t idx0, Fp* out, long long stride, long long elem_stride,
               int count, int B);
 
@@ -60,5 +62,10 @@ void powers(Ctx* c, Fp* out, long long out_stride, const Fp* x, long long x_stri
 enum ScalarOp { S_MUL = 0, S_ADD, S_SUB, S_INV, S_COPY, S_POW2K /* dst = a^(2^imm) */, S_CONST /* dst = consts[imm] */, S_NEG, S_FMA /* dst = dst*a + b */, S_POWI /* dst = a^imm */ };
 struct ScalarInstr { uint16_t op, dst, a, b; uint32_t imm; };
 void scalar_program(Ctx* c, Fp* vars, long long stride, const ScalarInstr* d_prog, int ninstr, const Fp* d_consts, int B);
+
+// ---------------------------------------------------------------- verifier.cu
+// The g-term of K proofs added into a batch's scalars (tb_batch_verifier): G[t] += sum_p (ab[2p] * s_{p,t} + [t = 0] ab[2p + 1])
+// for t < 2^kk, s_{p,t} = prod_j us[p * kk + j]^{bit_(kk-1-j)(t)}.  Montgomery form throughout.
+void batch_g_scalars(Ctx* c, Fp* G, const Fp* us, const Fp* ab, int kk, int K);
 
 }  // namespace tb

@@ -6,7 +6,8 @@
 // Accept iff   sum_i coef_i * C_i  +  xi*S  +  sum_j (u_j^-1 L_j + u_j R_j)  -  sum_t (c s_t + [t=0] v) g_t  -  (c b z) U  -  f W  ==  O
 // where the C_i are every commitment of the proof, of the verifying key and of the instance, with the multiopen
 // coefficients (SURVEY App. A.2/A.4).  The g-term is one fixed-base MSM over the SRS tables (U and W are its two extra
-// table columns), the rest a ~100-term variable-base MSM per proof.
+// table columns), the rest a ~100-term variable-base MSM per proof.  The batch verifier (tb_batch_verifier) sums these checks
+// with random weights over any number of proofs and circuits: one shared g-term, one variable-base MSM per call.
 #define TB_NOINLINE_MUL 1
 #include <algorithm>
 #include <cstdlib>
@@ -83,15 +84,32 @@ struct EvalView {
   Fp z_last(int s) const { return ev[{{PK_PZ, s}, last_rot}]; }
 };
 
-// n_proofs proofs of the circuit of shape C, whose fixed / sigma commitments are `vk_fixed` / `vk_sigma` (Montgomery)
-static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
-                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
+// sum(instance_len); refuses an instance column longer than the usable rows (InstanceTooLarge)
+static size_t instance_total(const Shape& C, const uint32_t* instance_len) {
+  size_t total = 0;
+  for (uint32_t c = 0; c < C.ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); total += instance_len[c]; }
+  return total;
+}
+
+// What the transcript replay of K proofs leaves for their final IPA checks.  Proof p's variable-base terms are pts / sc at
+// [p * stride, p * stride + M), unused slots the identity times 0.  With `wu_terms` the last two of them are W and U with
+// their scalars -f and -c*b*z and stride = M; otherwise stride is M rounded up to a power of two.  extras[p] = (-f, -c*b*z)
+// either way, us[p] = the kk IPA challenges u_j, cv[p] = (c, v).  alive[p] = 0 for a proof rejected during the replay (a read
+// that fails, an identity absorbed, a non-canonical scalar or instance value, trailing bytes); its terms are all unused.
+struct Replay {
+  int M = 0, stride = 0;
+  std::vector<Aff<Fq>> pts; std::vector<Fp> sc, us, cv, extras; std::vector<char> alive;
+};
+
+// Replays the transcripts of K proofs of proof_len == C.proof_len bytes of the circuit of shape C, whose fixed / sigma
+// commitments are `vk_fixed` / `vk_sigma` (Montgomery).  Every point is decoded and every instance column committed on the
+// device first.
+static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
+                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len,
+                         bool wu_terms, Replay& rep) {
   const size_t n = C.n; const int kk = (int)C.k, na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf, nf = C.nf, pieces = C.pieces;
   cudaStream_t st = ctx->stream;
-  size_t inst_total = 0;
-  for (int c = 0; c < ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); inst_total += instance_len[c]; }
-  for (int p = 0; p < K; ++p) ok_out[p] = 0;
-  if (proof_len != C.proof_len) return;   // no proof of this length is accepted
+  const size_t inst_total = instance_total(C, instance_len);
   // ---- every point of the batch, decoded on the device: [K][npts]
   const int npts = (int)C.point_offsets.size();
   std::vector<Aff<Fq>> dec((size_t)K * npts);
@@ -119,11 +137,12 @@ static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
   }
   // ---- per proof: replay the transcript, accumulate (scalar, point) pairs
   const int nps = (int)C.point_sets.size();
-  const int M = ni + na + 3 * L + nsets + 1 + pieces + nf + P + 2 + 2 * kk;   // variable-base terms per proof
-  int Mpad = 32; while (Mpad < M) Mpad *= 2;
-  std::vector<Aff<Fq>> vpts((size_t)K * Mpad, Aff<Fq>::inf());
-  std::vector<Fp> vsc((size_t)K * Mpad, Fp::zero()), us((size_t)K * kk, Fp::zero()), cv((size_t)K * 2, Fp::zero()), extras((size_t)K * 2, Fp::zero());
-  std::vector<char> alive(K, 0);
+  rep.M = ni + na + 3 * L + nsets + 1 + pieces + nf + P + 2 + 2 * kk + (wu_terms ? 2 : 0);   // variable-base terms per proof
+  if (wu_terms) rep.stride = rep.M;
+  else { rep.stride = 32; while (rep.stride < rep.M) rep.stride *= 2; }
+  rep.pts.assign((size_t)K * rep.stride, Aff<Fq>::inf());
+  rep.sc.assign((size_t)K * rep.stride, Fp::zero()); rep.us.assign((size_t)K * kk, Fp::zero()); rep.cv.assign((size_t)K * 2, Fp::zero()); rep.extras.assign((size_t)K * 2, Fp::zero());
+  rep.alive.assign(K, 0);
   const Fp one = Fp::one();
   const int last_rot = -(bf + 1);
   Fp omega = C.omega, omega_inv = C.omega.inv(), n_inv = Fp::from_u32((uint32_t)n).inv();
@@ -220,7 +239,7 @@ static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     if (!ok || tr.bad || tr.pos != proof_len) continue;
     Fp b = one; { Fp cur = x3; for (int j = kk - 1; j >= 0; --j) { b = b * (one + uj[j] * cur); cur = cur * cur; } }
     // ---- variable-base terms
-    Aff<Fq>* pp = vpts.data() + (size_t)p * Mpad; Fp* ss = vsc.data() + (size_t)p * Mpad; int w = 0;
+    Aff<Fq>* pp = rep.pts.data() + (size_t)p * rep.stride; Fp* ss = rep.sc.data() + (size_t)p * rep.stride; int w = 0;
     auto push = [&](const Aff<Fq>& pt, const Fp& sc) { pp[w] = pt; ss[w] = sc; ++w; };
     for (size_t c = 0; c < C.uniq.size(); ++c) {
       const PolyId& id = C.uniq[c]; Fp coef = coef_in_set[id] * x4pow[nps - 1 - C.uniq_set[c]];
@@ -232,18 +251,31 @@ static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     push(q_prime, x4pow[nps]);
     push(s_comm, xi);
     for (int j = 0; j < kk; ++j) { push(Ls[j], uj[j].inv()); push(Rs[j], uj[j]); }
-    if (w > Mpad) throw std::runtime_error("internal error: verifier term count");
-    for (int j = 0; j < kk; ++j) us[(size_t)p * kk + j] = uj[j];
-    cv[2 * p] = cc; cv[2 * p + 1] = v;
-    extras[2 * p] = ff.neg();                    // * W
-    extras[2 * p + 1] = (cc * b * z).neg();      // * U
-    alive[p] = 1;
+    rep.extras[2 * p] = ff.neg();                    // * W
+    rep.extras[2 * p + 1] = (cc * b * z).neg();      // * U
+    if (wu_terms) { push(srs.w_host, rep.extras[2 * p]); push(srs.u_host, rep.extras[2 * p + 1]); }
+    if (w > rep.stride) throw std::runtime_error("internal error: verifier term count");
+    for (int j = 0; j < kk; ++j) rep.us[(size_t)p * kk + j] = uj[j];
+    rep.cv[2 * p] = cc; rep.cv[2 * p + 1] = v;
+    rep.alive[p] = 1;
   }
-  // ---- device: both MSMs for the whole batch, then the identity test
-  DevBuf<Aff<Fq>> d_pts(ctx, vpts.size()); DevBuf<Fp> d_sc(ctx, vsc.size()), d_us(ctx, us.size()), d_cv(ctx, cv.size()), d_ex(ctx, extras.size()), d_gs(ctx, (size_t)K * n);
+}
+
+// n_proofs proofs of the circuit of shape C, each checked on its own: the replay, then both MSMs of every proof's final
+// check for the whole batch on the device, then the identity test
+static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
+                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
+  const size_t n = C.n; const int kk = (int)C.k;
+  instance_total(C, instance_len);
+  for (int p = 0; p < K; ++p) ok_out[p] = 0;
+  if (proof_len != C.proof_len) return;   // no proof of this length is accepted
+  Replay r;
+  replay_batch(ctx, C, srs, vk_fixed, vk_sigma, K, instance, instance_len, proofs, proof_stride, proof_len, false, r);
+  const int Mpad = r.stride;
+  DevBuf<Aff<Fq>> d_pts(ctx, r.pts.size()); DevBuf<Fp> d_sc(ctx, r.sc.size()), d_us(ctx, r.us.size()), d_cv(ctx, r.cv.size()), d_ex(ctx, r.extras.size()), d_gs(ctx, (size_t)K * n);
   DevBuf<Xyzz<Fq>> acc_v(ctx, K), acc_g(ctx, K); DevBuf<uint8_t> d_ok(ctx, K);
-  d_pts.upload(vpts.data(), vpts.size()); d_sc.upload(vsc.data(), vsc.size()); d_us.upload(us.data(), us.size()); d_cv.upload(cv.data(), cv.size());
-  d_ex.upload(extras.data(), extras.size());
+  d_pts.upload(r.pts.data(), r.pts.size()); d_sc.upload(r.sc.data(), r.sc.size()); d_us.upload(r.us.data(), r.us.size()); d_cv.upload(r.cv.data(), r.cv.size());
+  d_ex.upload(r.extras.data(), r.extras.size());
   MsmConfig cfg;
   msm_run<Fq, Fp>(ctx, d_sc.get(), (long long)Mpad, d_pts.get(), (long long)Mpad, Mpad, K, cfg, acc_v.get());
   launch(ctx, verify_g_scalars_kernel, dim3((unsigned)((n + 255) / 256), K), 256, 0, d_us.get(), d_cv.get(), d_gs.get(), kk, (int)n);
@@ -251,7 +283,119 @@ static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
   launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K);
   std::vector<uint8_t> hok(K);
   d_ok.download(hok.data(), K); ctx->sync();
-  for (int p = 0; p < K; ++p) ok_out[p] = (alive[p] && hok[p]) ? 1 : 0;
+  for (int p = 0; p < K; ++p) ok_out[p] = (r.alive[p] && hok[p]) ? 1 : 0;
+}
+
+// ---------------------------------------------------------------- batch verifier (tb_batch_verifier)
+// halo2's BatchVerifier: proof j's final-check sum is weighted by rho_j = PRF(seed, j, R_BATCH_WEIGHT, 0) and the weighted sums
+// of every proof added are added up, so one test for the identity decides the whole batch.  All proofs commit over one SRS,
+// so their g-terms share `g` (n scalars); everything else of a call's proofs goes through one variable-base MSM whose result
+// is added into `acc`.  `next` is the j of the next proof; `rejected`: a proof was rejected before its final check.
+struct BatchVerifier {
+  const Srs* srs = nullptr; int device = 0; uint8_t seed[32];
+  uint64_t next = 0;
+  bool rejected = false;
+  bool broken = false;      // an add failed after it began changing g / acc: only tb_batch_verifier_free is allowed
+  bool finalized = false;
+  DevMem<Fp> g;             // [n] sum_p rho_p (-c_p s_{p,t} - [t = 0] v_p), Montgomery
+  DevMem<Xyzz<Fq>> acc;     // [1] sum_p rho_p (every variable-base term of proof p, W and U included)
+};
+
+// Per proof p of a call (one CTA each): its M variable-base scalars times rho_p, and ab[p] = (-rho_p c_p, -rho_p v_p), the
+// coefficients of its g-term.
+__global__ void batch_weights_kernel(const Fp* __restrict__ rho, Fp* __restrict__ sc, int M, const Fp* __restrict__ cv, Fp* __restrict__ ab) {
+  const int p = blockIdx.x;
+  const Fp w = ldg_fe(rho + p);
+  if (threadIdx.x < 2) st_fe(ab + 2 * p + threadIdx.x, (w * ldg_fe(cv + 2 * p + threadIdx.x)).neg());
+  for (int i = threadIdx.x; i < M; i += blockDim.x) { Fp* s = sc + (size_t)p * M + i; st_fe(s, ld_fe(s) * w); }
+}
+
+__global__ void batch_acc_kernel(Xyzz<Fq>* acc, const Xyzz<Fq>* add) {
+  Xyzz<Fq> s = *acc; s.add(*add); *acc = s;
+}
+
+// G[t] += sum_p (a_p s_{p,t} + [t = 0] b_p), s_{p,t} = prod_j u_{p,j}^{bit_(kk-1-j)(t)}, (a_p, b_p) = ab[p].  With t = hi * 2^lb
+// + lo (lb = min(kk, BG_LOG)), s_{p,t} = H_p(hi) * L_p(lo), H over the top kk - lb bits, L over the low lb bits.  One CTA per
+// hi: for BG_PROOFS proofs at a time it writes a_p H_p(hi) into entry 0 of a table in shared memory and doubles the table lb
+// times (entries [m, 2m) = entries [0, m) times the u of bit log2(m)), which leaves a_p s_{p,t} in entry lo; each thread then
+// adds its entries.  One product per (proof, t), plus ~(kk - lb)/2 per (proof, CTA) for H.
+constexpr int BG_LOG = 8, BG_THREADS = 1 << BG_LOG, BG_PROOFS = 4;
+__global__ void __launch_bounds__(BG_THREADS) batch_g_scalars_kernel(Fp* __restrict__ G, const Fp* __restrict__ us, const Fp* __restrict__ ab, int kk, int K) {
+  __shared__ Fp tab[BG_PROOFS][BG_THREADS];
+  const int lb = kk < BG_LOG ? kk : BG_LOG, lo = threadIdx.x;
+  const uint32_t hi = blockIdx.x;
+  Fp acc = Fp::zero();
+  for (int p0 = 0; p0 < K; p0 += BG_PROOFS) {
+    const int np = K - p0 < BG_PROOFS ? K - p0 : BG_PROOFS;
+    if (lo < np) {
+      const Fp* u = us + (size_t)(p0 + lo) * kk;
+      Fp h = ldg_fe(ab + 2 * (p0 + lo));
+      for (int j = 0; j < kk - lb; ++j) if ((hi >> (kk - lb - 1 - j)) & 1) h = h * ldg_fe(u + j);
+      tab[lo][0] = h;
+    }
+    __syncthreads();
+    for (int b = 0; b < lb; ++b) {
+      for (int e = threadIdx.x; e < (np << b); e += BG_THREADS) {
+        const int q = e >> b, i = e & ((1 << b) - 1);
+        tab[q][(1 << b) + i] = tab[q][i] * ldg_fe(us + (size_t)(p0 + q) * kk + kk - 1 - b);
+      }
+      __syncthreads();
+    }
+    if (lo < (1 << lb)) for (int q = 0; q < np; ++q) acc = acc + tab[q][lo];
+    if (hi == 0 && lo == 0) for (int q = 0; q < np; ++q) acc = acc + ldg_fe(ab + 2 * (p0 + q) + 1);
+    __syncthreads();
+  }
+  if (lo < (1 << lb)) { Fp* g = G + ((size_t)hi << lb) + lo; st_fe(g, ld_fe(g) + acc); }
+}
+
+void batch_g_scalars(Ctx* ctx, Fp* G, const Fp* us, const Fp* ab, int kk, int K) {
+  TB_REQUIRE(kk >= 1 && kk <= 30 && K >= 1, "batch_g_scalars shape");
+  const int lb = kk < BG_LOG ? kk : BG_LOG;
+  ProfScope scope(ctx, PC_IPA_FOLD);
+  ctx->work[PC_IPA_FOLD] += (double)K * (double)(1ull << kk) * (1.0 + 0.5 * (kk - lb) / (1 << lb));
+  launch(ctx, batch_g_scalars_kernel, (unsigned)(1u << (kk - lb)), BG_THREADS, 0, G, us, ab, kk, K);
+}
+
+// The proofs of one tb_batch_verifier_add: replay, then (unless a proof was rejected) their weights, their terms through one
+// variable-base MSM into bv.acc, and their g-terms into bv.g.
+static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K, const uint8_t* instance, const uint32_t* instance_len,
+                      const uint8_t* proofs, size_t proof_stride, size_t proof_len) {
+  const Shape& C = vk.shape;
+  const uint32_t j0 = (uint32_t)bv.next;
+  if (!bv.rejected && proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted
+  if (!bv.rejected) {
+    Replay r;
+    replay_batch(ctx, C, *vk.srs, vk.fixed, vk.sigma, K, instance, instance_len, proofs, proof_stride, proof_len, true, r);
+    if (std::find(r.alive.begin(), r.alive.end(), 0) != r.alive.end()) bv.rejected = true;
+    else {
+      const size_t N = (size_t)K * r.M;
+      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_cv(ctx, r.cv.size()), d_rho(ctx, K), d_ab(ctx, 2 * (size_t)K);
+      DevBuf<Xyzz<Fq>> part(ctx, 1);
+      d_pts.upload(r.pts.data(), N); d_sc.upload(r.sc.data(), N); d_us.upload(r.us.data(), r.us.size()); d_cv.upload(r.cv.data(), r.cv.size());
+      bv.broken = true;
+      { ProfScope scope(ctx, PC_IPA_FOLD);
+        prf_fill(ctx, bv.seed, j0, R_BATCH_WEIGHT, 0, d_rho.get(), 1, 1, 1, K);
+        ctx->work[PC_IPA_FOLD] += (double)K * (r.M + 2);
+        launch(ctx, batch_weights_kernel, K, 128, 0, d_rho.get(), d_sc.get(), r.M, d_cv.get(), d_ab.get()); }
+      msm_run<Fq, Fp>(ctx, d_sc.get(), 0, d_pts.get(), 0, (int)N, 1, MsmConfig(), part.get());
+      { ProfScope scope(ctx, PC_MSM_REDUCE);
+        launch(ctx, batch_acc_kernel, 1, 1, 0, bv.acc.get(), part.get()); }
+      batch_g_scalars(ctx, bv.g.get(), d_us.get(), d_ab.get(), (int)C.k, K);
+      ctx->sync();   // the batch may be used from another context (stream) next
+      bv.broken = false;
+    }
+  }
+  bv.next += (uint64_t)K;
+}
+
+// 1 iff the weighted sum of every final check added is the identity: g through the SRS's fixed-base tables, plus acc
+static uint8_t batch_finalize(Ctx* ctx, const BatchVerifier& bv) {
+  DevBuf<Xyzz<Fq>> acc_g(ctx, 1); DevBuf<uint8_t> d_ok(ctx, 1);
+  bv.srs->commit_xyzz(ctx, false, bv.g.get(), (long long)bv.srs->n, 1, nullptr, 0, acc_g.get());
+  launch(ctx, verify_final_kernel, 1, 32, 0, bv.acc.get(), acc_g.get(), d_ok.get(), 1);
+  uint8_t ok = 0;
+  d_ok.download(&ok, 1); ctx->sync();
+  return ok;
 }
 
 // The verifying key of a proving key: commit_lagrange(column, Blind::default()) of every fixed and sigma column, computed on
@@ -328,6 +472,58 @@ tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proofs, c
   verify_batch(&ctx->c, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
   TB_API_END(ctx)
 }
+
+tb_status tb_batch_verifier_create(tb_ctx* ctx, const tb_srs* srs_, const uint8_t seed[32], tb_batch_verifier** out) {
+  TB_API_BEGIN(ctx)
+  const Srs* srs = reinterpret_cast<const Srs*>(srs_);
+  TB_REQUIRE(srs && seed && out, "tb_batch_verifier_create arguments");
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  std::unique_ptr<BatchVerifier> bv(new BatchVerifier());
+  bv->srs = srs; bv->device = ctx->c.device; memcpy(bv->seed, seed, 32);
+  bv->g = DevMem<Fp>(srs->n);
+  bv->acc = DevMem<Xyzz<Fq>>(1);
+  // zero bytes: the scalar 0 (Montgomery) and the XYZZ identity
+  TB_CUDA(cudaMemsetAsync(bv->g.get(), 0, srs->n * sizeof(Fp), ctx->c.stream));
+  TB_CUDA(cudaMemsetAsync(bv->acc.get(), 0, sizeof(Xyzz<Fq>), ctx->c.stream));
+  ctx->c.sync();
+  *out = reinterpret_cast<tb_batch_verifier*>(bv.release());
+  TB_API_END(ctx)
+}
+
+tb_status tb_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv_, const tb_vk* vk_, uint32_t n_proofs, const uint8_t* instance,
+                                const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len) {
+  TB_API_BEGIN(ctx)
+  BatchVerifier* bv = reinterpret_cast<BatchVerifier*>(bv_);
+  const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
+  // every refusal comes before the batch changes
+  TB_REQUIRE(bv && vk && n_proofs >= 1 && n_proofs <= 4096 && proofs && proof_stride >= proof_len && (vk->shape.ni == 0 || (instance && instance_len)),
+             "tb_batch_verifier_add arguments");
+  TB_REQUIRE(!bv->finalized, "tb_batch_verifier_add after tb_batch_verifier_finalize");
+  TB_REQUIRE(!bv->broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
+  TB_REQUIRE(vk->srs == bv->srs, "the verifying key refers to another SRS than the batch");
+  TB_REQUIRE(ctx->c.device == bv->device, "the context is on another device than the batch");
+  TB_REQUIRE(bv->next + n_proofs <= (1ull << 32), "a batch holds at most 2^32 proofs");
+  instance_total(vk->shape, instance_len);
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  batch_add(&ctx->c, *bv, *vk, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len);
+  TB_API_END(ctx)
+}
+
+tb_status tb_batch_verifier_finalize(tb_ctx* ctx, tb_batch_verifier* bv_, uint8_t* ok_out) {
+  TB_API_BEGIN(ctx)
+  BatchVerifier* bv = reinterpret_cast<BatchVerifier*>(bv_);
+  TB_REQUIRE(bv && ok_out, "tb_batch_verifier_finalize arguments");
+  TB_REQUIRE(!bv->finalized, "tb_batch_verifier_finalize after tb_batch_verifier_finalize");
+  TB_REQUIRE(!bv->broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
+  TB_REQUIRE(ctx->c.device == bv->device, "the context is on another device than the batch");
+  bv->finalized = true;
+  *ok_out = 0;
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  if (!bv->rejected) *ok_out = batch_finalize(&ctx->c, *bv);
+  TB_API_END(ctx)
+}
+
+void tb_batch_verifier_free(tb_batch_verifier* bv) { delete reinterpret_cast<BatchVerifier*>(bv); }
 
 tb_status tb_decompress(tb_ctx* ctx, size_t n, const uint8_t* in, uint8_t* out, uint8_t* ok) {
   TB_API_BEGIN(ctx)

@@ -64,6 +64,10 @@ _SIGS = {
     "tb_vk_proof_len": (_sz, [_vp]),
     "tb_verify_batch_vk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
     "tb_check_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp]),
+    "tb_batch_verifier_create": (_i, [_vp, _vp, _vp, ctypes.POINTER(_vp)]),
+    "tb_batch_verifier_add": (_i, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz]),
+    "tb_batch_verifier_finalize": (_i, [_vp, _vp, _vp]),
+    "tb_batch_verifier_free": (None, [_vp]),
 }
 
 TB_FAIL_GATE, TB_FAIL_LOOKUP, TB_FAIL_COPY = 1, 2, 3
@@ -395,6 +399,50 @@ class VerifyingKey:
     def close(self):
         if getattr(self, "_h", None):
             self.ctx._lib.tb_vk_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class BatchVerifier:
+    """halo2's plonk::BatchVerifier over the device (tb_batch_verifier): proofs of any circuits whose verifying keys refer to
+    `srs`, added in any number of calls, then one verdict from finalize().  `seed` (32 bytes) draws the proofs' random weights;
+    it must be unpredictable to whoever made the proofs: draw a fresh one per batch."""
+
+    def __init__(self, srs, seed):
+        self.srs, self.ctx = srs, srs.ctx
+        seed = _u8(np.frombuffer(bytes(seed), np.uint8))
+        assert seed.size == 32
+        h = _vp()
+        self.ctx._check(self.ctx._lib.tb_batch_verifier_create(self.ctx._h, srs._h, _ptr(seed), ctypes.byref(h)))
+        self._h = h
+
+    def add(self, vk, instance, instance_len, proofs, ctx=None):
+        """add_proof for each of `proofs` (byte strings of one length, at most 4096) of vk's circuit; instance / instance_len
+        as in VerifyingKey.verify_batch.  A proof that fails before its final check makes finalize() False."""
+        ctx = ctx or self.ctx
+        B = len(proofs)
+        plen = len(proofs[0]) if B else 0
+        assert all(len(p) == plen for p in proofs)
+        buf = np.frombuffer(b"".join(proofs), np.uint8).copy() if B else np.zeros(1, np.uint8)
+        inst = _u8(instance)
+        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+        ctx._check(ctx._lib.tb_batch_verifier_add(ctx._h, self._h, vk._h, B, _ptr(inst), _ptr(lens), _ptr(buf), plen, plen))
+
+    def finalize(self, ctx=None):
+        """True iff every proof added would be accepted by VerifyingKey.verify_batch.  Consumes the batch."""
+        ctx = ctx or self.ctx
+        ok = np.zeros(1, np.uint8)
+        ctx._check(ctx._lib.tb_batch_verifier_finalize(ctx._h, self._h, _ptr(ok)))
+        return bool(ok[0])
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self.ctx._lib.tb_batch_verifier_free(self._h)
             self._h = None
 
     def __del__(self):

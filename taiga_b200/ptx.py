@@ -132,6 +132,38 @@ class ProverService:
                     out[i // per].append((name, i % per, counts, [lib.render_failure(pk.keydata, f) for f in fails]))
         return out
 
+    def verifying_keys(self):
+        """(Compliance vk, VP vk), built once from the proving keys."""
+        if getattr(self, "_vks", None) is None:
+            self._vks = (self.pk_c.verifying_key(), self.pk_v.verifying_key())
+        return self._vks
+
+    def verify_ptx_batch(self, c_proofs, v_proofs, wit, seed, max_batch=4096):
+        """The proof part of ShieldedPartialTxBundle::execute (shielded_ptx.rs:137-153) for the partial transactions of
+        `wit` (what synthesize_ptx returns): every Compliance and VP proof goes into one BatchVerifier, finalized once.  `seed`
+        (32 bytes) must be unpredictable to whoever made the proofs.  Returns (all accepted, [verdict per partial transaction]);
+        when the batch is rejected, each circuit's proofs are verified one by one to name the failing partial transactions."""
+        n_ptx = len(wit["c_inst"]) // COMPLIANCE_PER_PTX
+        assert len(c_proofs) == COMPLIANCE_PER_PTX * n_ptx and len(v_proofs) == VP_PER_PTX * n_ptx
+        circuits = [(vk, proofs, inst, lens, per) for vk, proofs, inst, lens, per in
+                    zip(self.verifying_keys(), (c_proofs, v_proofs), (wit["c_inst"], wit["v_inst"]), (wit["c_len"], wit["v_len"]),
+                        (COMPLIANCE_PER_PTX, VP_PER_PTX))]
+        bv = lib.BatchVerifier(self.srs, seed)
+        try:
+            for vk, proofs, inst, lens, _ in circuits:
+                for lo in range(0, len(proofs), max_batch):
+                    bv.add(vk, inst[lo:lo + max_batch], lens, proofs[lo:lo + max_batch])
+            if bv.finalize():
+                return True, [True] * n_ptx
+        finally:
+            bv.close()
+        verdicts = [True] * n_ptx
+        for vk, proofs, inst, lens, per in circuits:
+            for lo in range(0, len(proofs), max_batch):
+                for i, ok in enumerate(vk.verify_batch(inst[lo:lo + max_batch], lens, proofs[lo:lo + max_batch]), lo):
+                    verdicts[i // per] &= ok
+        return all(verdicts), verdicts
+
     @property
     def launch_count(self):
         return sum(c.launch_count for c in self.contexts)

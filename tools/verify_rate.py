@@ -7,6 +7,8 @@ Reports, fastest of --repeats calls:
     the per-proof variable-base MSM and the fixed-base g term), and the rest of the wall time: the host replay, the copies
     and the few small kernels outside the profiler's categories (the calls synchronise between phases, so host and device
     time do not overlap);
+  * the batch verifier (tb_batch_verifier): the same 384 proofs in one batch, both circuits, one finalize, with the same
+    split into device MSMs and the rest;
   * the old path, which decoded every point on the host: the same points through the host build of the same decoder
     (tests/host_shim.cpp, g++ -O2, one thread), and the wall time that path would take (vk wall - device decode + host decode).
 
@@ -106,7 +108,7 @@ def main():
         circuits.append((kd, pk, proofs, inst, lens))
     n_proofs = sum(len(c[2]) for c in circuits)
     pk_s = best(lambda: [pk.verify_batch(inst, lens, proofs) for _, pk, proofs, inst, lens in circuits], args.repeats)
-    res = {"proofs": n_proofs, "gpu": _gpu_name(), "pk_seconds": round(pk_s, 4), "pk_proofs_per_s": round(n_proofs / pk_s, 1)}
+    res = {"proofs": n_proofs, "gpu": _gpu_name(), "power_limit": _power_limit(), "pk_seconds": round(pk_s, 4), "pk_proofs_per_s": round(n_proofs / pk_s, 1)}
     if args.tree:
         res["lib"] = lib.LIB_PATH
         print(json.dumps(res))
@@ -133,6 +135,26 @@ def main():
           % (n_proofs, vk_s * 1e3, n_proofs / vk_s, decode_ms, msm_ms, vk_s * 1e3 - device_ms))
     print("host decoding of the same %d points: %.1f ms (%.1f us/point): that path would take %.1f ms (%.0f proofs/s)"
           % (len(points), host_dec * 1e3, host_dec * 1e6 / len(points), old_s * 1e3, n_proofs / old_s))
+    # the batch verifier: one batch of both circuits, one finalize
+    def batch():
+        bv = lib.BatchVerifier(srs, bytes(range(7, 39)))
+        for vk, c in zip(vks, circuits):
+            bv.add(vk, c[3], c[4], c[2])
+        ok = bv.finalize()
+        bv.close()
+        return [[ok]]
+    bv_s = best(batch, args.repeats)
+    ctx.prof_enable(True)
+    batch()
+    prof = ctx.prof_read()
+    ctx.prof_enable(False)
+    bv_msm_ms = sum(prof[k][0] for k in ("msm_sort", "msm_accum", "msm_reduce"))
+    bv_other_ms = prof["transcript"][0] + prof["ipa_fold"][0]
+    res.update({"batch_seconds": round(bv_s, 4), "batch_proofs_per_s": round(n_proofs / bv_s, 1), "batch_device_msm_ms": round(bv_msm_ms, 2),
+                "batch_device_decode_weights_g_ms": round(bv_other_ms, 3), "batch_host_replay_and_copies_ms": round(bv_s * 1e3 - bv_msm_ms - bv_other_ms, 1)})
+    print("tb_batch_verifier:  %d proofs in %.1f ms (%.0f proofs/s); device MSMs %.1f ms, device decode + weights + g-term %.2f ms, host replay and copies %.0f ms"
+          % (n_proofs, bv_s * 1e3, n_proofs / bv_s, bv_msm_ms, bv_other_ms, bv_s * 1e3 - bv_msm_ms - bv_other_ms))
+    print("measured on: %s, power limit %s" % (res["gpu"], res["power_limit"]))
     print(json.dumps(res))
     for vk in vks:
         vk.close()
@@ -142,6 +164,15 @@ def _gpu_name():
     try:
         import torch
         return torch.cuda.get_device_name(0)
+    except Exception:
+        return "?"
+
+
+def _power_limit():
+    """the enforced power limit of GPU 0, as nvidia-smi reports it (a read-only query)"""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return r.stdout.strip() or "?"
     except Exception:
         return "?"
 
