@@ -139,7 +139,7 @@ static void check_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   const size_t n = C.n; const long long nn = (long long)n;
   const int na = C.na, ni = C.ni, L = C.L, P = C.P, U = (int)C.usable, J = (int)C.plan.num_constraints;
   const int ni1 = std::max(1, ni), L1 = std::max(1, L), P1 = std::max(1, P);
-  witness_instance_total(C, instance_len);
+  instance_total(C, instance_len);
   check_prepare(C);
   ProveWs* claimed = C.claim_workspace(ctx, B, true);
   TB_REQUIRE(claimed != nullptr, "this proving key / context / batch size is already checking on another thread (a tb_ctx is bound to one thread)");

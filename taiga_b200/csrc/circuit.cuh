@@ -15,6 +15,7 @@ namespace tb {
 enum PolyKind { PK_INST = 0, PK_ADV, PK_PZ, PK_LZ, PK_LPIN, PK_LPTAB, PK_FIXED, PK_SIG, PK_H, PK_RANDOM };
 struct PolyId { int kind, idx; bool operator<(const PolyId& o) const { return kind != o.kind ? kind < o.kind : idx < o.idx; } bool operator==(const PolyId& o) const { return kind == o.kind && idx == o.idx; } };
 struct QueryRef { PolyId poly; int rot; };
+inline PolyId column_poly(const tb_column& col) { return {col.kind == TB_COL_ADVICE ? PK_ADV : col.kind == TB_COL_FIXED ? PK_FIXED : PK_INST, (int)col.index}; }
 // Scratch of one (context, batch size) pair: device blocks in request order and the small tables uploaded on first use.
 // A tb_pk may be shared by several contexts (= host threads); each gets its own workspace, and a second thread entering
 // with the SAME context and batch size while a call is in flight is refused (TB_ERR_INVALID) instead of corrupting it.
@@ -32,6 +33,14 @@ struct Shape {
   Fp delta_c0[PERM_MAX_SETS];
   // evaluation / multiopen structure
   std::vector<QueryRef> evals;            // transcript order of the evaluation section
+  // (poly, rotation) -> its position in `evals` (the last one, should a query repeat); (PK_H, 0) -> evals.size(), where the
+  // verifier keeps the h(x) it expects.  Every permutation column has its rotation-0 query (shape_build refuses it otherwise).
+  std::map<std::pair<PolyId, int>, int> eval_pos;
+  int eval_index(const PolyId& poly, int rot) const {
+    auto it = eval_pos.find({poly, rot});
+    if (it == eval_pos.end()) throw std::logic_error("internal error: a query without an evaluation");
+    return it->second;
+  }
   std::vector<QueryRef> queries;          // multiopen query order
   std::vector<int> rots;                  // distinct rotations (evaluation points), in order of first appearance in `queries`
   std::vector<PolyId> uniq; std::vector<int> uniq_set; std::vector<std::vector<int>> point_sets;
@@ -109,11 +118,15 @@ struct WsAlloc {
 };
 
 
-// The witness of B proofs on the device in Montgomery form (Lagrange basis), shared by the prover and the check:
-// instance columns [B][ni][n] zero past instance_len, advice [B][na][n] (host or device pointer) whose rows >= usable are
-// overwritten with PRF(seed, proof0 + b, rows_tag, c * (bf + 1) + r - usable).  Refuses an instance column longer than the
-// usable rows (InstanceTooLarge); witness_instance_total checks that alone and returns sum(instance_len).
-size_t witness_instance_total(const Circuit& C, const uint32_t* instance_len);
+// sum(instance_len); refuses an instance column longer than the usable rows (InstanceTooLarge)
+size_t instance_total(const Shape& C, const uint32_t* instance_len);
+// The instance columns of B proofs on the device in Montgomery form (Lagrange basis), [B][ni][n] zero past instance_len;
+// `instance` holds each proof's sum(instance_len) values column after column; refuses what instance_total refuses.  Shared by
+// the prover, the check and the verifier.
+void upload_instance(Ctx* ctx, const Shape& C, int B, const uint8_t* instance, const uint32_t* instance_len, Fp* dst);
+// The witness of B proofs on the device in Montgomery form (Lagrange basis), shared by the prover and the check: the
+// instance columns as upload_instance leaves them, advice [B][na][n] (host or device pointer) whose rows >= usable are
+// overwritten with PRF(seed, proof0 + b, rows_tag, c * (bf + 1) + r - usable).
 void upload_witness(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,
                     const uint8_t* seed, uint32_t proof0, uint32_t rows_tag, Fp* inst_vals, Fp* adv_vals);
 

@@ -69,7 +69,11 @@ tb_status tbp_lookup_arrange(tb_ctx* ctx, const void* sorted_a, const void* sort
 }
 // the batch verifier's g-term (verifier.cu): G (2^kk scalars) += the terms of K proofs, us [K][kk], ab [K][2]
 tb_status tbp_batch_g_scalars(tb_ctx* ctx, void* G, const void* us, const void* ab, int kk, int K) {
-  TB_API_BEGIN(ctx) batch_g_scalars(&ctx->c, FP(G), CFP(us), CFP(ab), kk, K); TB_API_END(ctx)
+  TB_API_BEGIN(ctx) batch_g_scalars(&ctx->c, FP(G), CFP(us), CFP(ab), kk, K, K); TB_API_END(ctx)
+}
+// the same driver with the proofs in groups of `group` (1: the per-proof verifier's call): G [ceil(K / group)][2^kk]
+tb_status tbp_batch_g_scalars_grouped(tb_ctx* ctx, void* G, const void* us, const void* ab, int kk, int K, int group) {
+  TB_API_BEGIN(ctx) batch_g_scalars(&ctx->c, FP(G), CFP(us), CFP(ab), kk, K, group); TB_API_END(ctx)
 }
 
 }  // extern "C"

@@ -144,29 +144,33 @@ struct Prog {
   std::vector<ScalarInstr> ins;
   void op(int o, int dst, int a = 0, int b = 0, uint32_t imm = 0) { ScalarInstr i; i.op = (uint16_t)o; i.dst = (uint16_t)dst; i.a = (uint16_t)a; i.b = (uint16_t)b; i.imm = imm; ins.push_back(i); }
 };
-size_t witness_instance_total(const Circuit& C, const uint32_t* instance_len) {
+size_t instance_total(const Shape& C, const uint32_t* instance_len) {
   size_t total = 0;
   for (uint32_t c = 0; c < C.ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); total += instance_len[c]; }
   return total;
 }
 
+void upload_instance(Ctx* ctx, const Shape& C, int B, const uint8_t* instance, const uint32_t* instance_len, Fp* dst) {
+  const size_t n = C.n, inst_total = instance_total(C, instance_len);
+  const int ni = C.ni;
+  if (!ni) return;
+  TB_CUDA(cudaMemsetAsync(dst, 0, (size_t)B * ni * n * sizeof(Fp), ctx->stream));
+  size_t off = 0;
+  for (int c = 0; c < ni; ++c) {
+    if (instance_len[c])
+      TB_CUDA(cudaMemcpy2DAsync(dst + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, B,
+                                cudaMemcpyHostToDevice, ctx->stream));
+    off += instance_len[c];
+  }
+  fe_to_mont<Fp>(ctx, dst, (size_t)B * ni * n);
+}
+
 void upload_witness(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,
                     const uint8_t* seed, uint32_t proof0, uint32_t rows_tag, Fp* inst_vals, Fp* adv_vals) {
-  const size_t n = C.n, inst_total = witness_instance_total(C, instance_len);
-  const int na = C.na, ni = C.ni, bf = C.bf;
-  cudaStream_t st = ctx->stream;
-  if (ni) {
-    TB_CUDA(cudaMemsetAsync(inst_vals, 0, (size_t)B * ni * n * sizeof(Fp), st));
-    size_t off = 0;
-    for (int c = 0; c < ni; ++c) {
-      if (instance_len[c])
-        TB_CUDA(cudaMemcpy2DAsync(inst_vals + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, B,
-                                  cudaMemcpyHostToDevice, st));
-      off += instance_len[c];
-    }
-    fe_to_mont<Fp>(ctx, inst_vals, (size_t)B * ni * n);
-  }
-  TB_CUDA(cudaMemcpyAsync(adv_vals, advice, (size_t)B * na * n * 32, cudaMemcpyDefault, st));  // host or device pointer
+  const size_t n = C.n;
+  const int na = C.na, bf = C.bf;
+  upload_instance(ctx, C, B, instance, instance_len, inst_vals);
+  TB_CUDA(cudaMemcpyAsync(adv_vals, advice, (size_t)B * na * n * 32, cudaMemcpyDefault, ctx->stream));  // host or device pointer
   fe_to_mont<Fp>(ctx, adv_vals, (size_t)B * na * n);
   for (int c = 0; c < na; ++c)
     prf_fill(ctx, seed, proof0, rows_tag, (uint32_t)(c * (bf + 1)), adv_vals + (size_t)c * n + C.usable, (long long)na * n, 1, bf + 1, B);
@@ -183,7 +187,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   const int O_ADV = 0, O_INST = na, O_PZ = na + ni, O_LZ = na + ni + nsets, O_LPIN = O_LZ + L, O_LPTAB = O_LZ + 2 * L;
   const long long PS = (long long)NC * nn;   // per-proof stride of the merged buffers
   cudaStream_t st = ctx->stream;
-  witness_instance_total(C, instance_len);
+  instance_total(C, instance_len);
   ProveWs* claimed = C.claim_workspace(ctx, B);
   TB_REQUIRE(claimed != nullptr, "this proving key / context / batch size is already proving on another thread (a tb_ctx is bound to one thread)");
   ProveWs& pws = *claimed;
@@ -603,27 +607,6 @@ tb_status tb_circuit_load(tb_ctx* ctx, const tb_srs* srs, const tb_cs_desc* cs, 
 }
 void tb_pk_free(tb_pk* pk) { delete reinterpret_cast<Circuit*>(pk); }
 
-// keygen_vk on the device: commit_lagrange(column, Blind::default() = 1) of every fixed and sigma column
-tb_status tb_pk_commitments(tb_ctx* ctx, const tb_pk* pk, uint8_t* fixed_commitments, uint8_t* sigma_commitments) {
-  TB_API_BEGIN(ctx)
-  const Circuit* C = reinterpret_cast<const Circuit*>(pk);
-  TB_REQUIRE(C && (fixed_commitments || C->nf == 0) && (sigma_commitments || C->P == 0), "tb_pk_commitments arguments");
-  TB_CUDA(cudaSetDevice(ctx->c.device));
-  Ctx* c = &ctx->c;
-  for (int which = 0; which < 2; ++which) {
-    int cnt = which ? (int)C->P : (int)C->nf;
-    if (!cnt) continue;
-    DevBuf<Fp> ones(c, cnt);
-    DevBuf<Aff<Fq>> pts(c, cnt);
-    std::vector<Fp> h(cnt, Fp::one());
-    ones.upload(h.data(), cnt);
-    C->srs->commit(c, true, which ? C->sig_vals.get() : C->fixed_vals.get(), (long long)C->n, cnt, ones.get(), pts.get());
-    fe_from_mont<Fq>(c, reinterpret_cast<Fq*>(pts.get()), 2 * (size_t)cnt);
-    pts.download(which ? sigma_commitments : fixed_commitments, cnt);
-    c->sync();
-  }
-  TB_API_END(ctx)
-}
 size_t tb_pk_proof_len(const tb_pk* pk) { return pk ? reinterpret_cast<const Circuit*>(pk)->proof_len : 0; }
 
 tb_status tb_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,

@@ -64,8 +64,9 @@ struct ScalarInstr { uint16_t op, dst, a, b; uint32_t imm; };
 void scalar_program(Ctx* c, Fp* vars, long long stride, const ScalarInstr* d_prog, int ninstr, const Fp* d_consts, int B);
 
 // ---------------------------------------------------------------- verifier.cu
-// The g-term of K proofs added into a batch's scalars (tb_batch_verifier): G[t] += sum_p (ab[2p] * s_{p,t} + [t = 0] ab[2p + 1])
-// for t < 2^kk, s_{p,t} = prod_j us[p * kk + j]^{bit_(kk-1-j)(t)}.  Montgomery form throughout.
-void batch_g_scalars(Ctx* c, Fp* G, const Fp* us, const Fp* ab, int kk, int K);
+// The g-terms of K proofs, added up per group of `group` consecutive proofs: G[g][t] += sum_{p in g} (ab[2p] * s_{p,t} + [t = 0]
+// ab[2p + 1]) for t < 2^kk, s_{p,t} = prod_j us[p * kk + j]^{bit_(kk-1-j)(t)}; G holds ceil(K / group) rows of 2^kk.  The batch
+// verifier adds all its proofs into one row, the per-proof verifier gives each proof its own.  Montgomery form throughout.
+void batch_g_scalars(Ctx* c, Fp* G, const Fp* us, const Fp* ab, int kk, int K, int group);
 
 }  // namespace tb

@@ -48,6 +48,14 @@ Shape shape_build(const tb_cs_desc* cs, uint32_t srs_k, bool allow_split) {
     C.evals.push_back({{PK_LZ, (int)l}, 0}); C.evals.push_back({{PK_LZ, (int)l}, 1}); C.evals.push_back({{PK_LPIN, (int)l}, 0});
     C.evals.push_back({{PK_LPIN, (int)l}, -1}); C.evals.push_back({{PK_LPTAB, (int)l}, 0});
   }
+  for (size_t i = 0; i < C.evals.size(); ++i) C.eval_pos[{C.evals[i].poly, C.evals[i].rot}] = (int)i;
+  C.eval_pos[{{PK_H, 0}, 0}] = (int)C.evals.size();
+  // the permutation argument reads every column at X: without that query its copy constraints would not bind the column
+  for (uint32_t c = 0; c < C.P; ++c) {
+    static const char* kinds[] = {"advice", "fixed", "instance"};
+    TB_REQUIRE(C.eval_pos.count({column_poly(C.perm[c]), 0}), "permutation column " + std::to_string(c) + " (" + kinds[C.perm[c].kind] + " column " +
+               std::to_string(C.perm[c].index) + ") has no rotation-0 query");
+  }
   for (auto& q : C.iq) C.queries.push_back({{PK_INST, (int)q.column}, q.rotation});
   for (auto& q : C.aq) C.queries.push_back({{PK_ADV, (int)q.column}, q.rotation});
   for (uint32_t s = 0; s < C.nsets; ++s) { C.queries.push_back({{PK_PZ, (int)s}, 0}); C.queries.push_back({{PK_PZ, (int)s}, 1}); }

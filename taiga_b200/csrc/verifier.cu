@@ -5,9 +5,9 @@
 // (taiga_halo2/src/proof.rs:45-54; serial loop over proofs in ShieldedPartialTxBundle::execute, transaction.rs:246-257).
 // Accept iff   sum_i coef_i * C_i  +  xi*S  +  sum_j (u_j^-1 L_j + u_j R_j)  -  sum_t (c s_t + [t=0] v) g_t  -  (c b z) U  -  f W  ==  O
 // where the C_i are every commitment of the proof, of the verifying key and of the instance, with the multiopen
-// coefficients (SURVEY App. A.2/A.4).  The g-term is one fixed-base MSM over the SRS tables (U and W are its two extra
-// table columns), the rest a ~100-term variable-base MSM per proof.  The batch verifier (tb_batch_verifier) sums these checks
-// with random weights over any number of proofs and circuits: one shared g-term, one variable-base MSM per call.
+// coefficients (SURVEY App. A.2/A.4).  The g-term is one fixed-base MSM over the SRS tables, the rest (W and U included) a
+// ~100-term variable-base MSM per proof.  The batch verifier (tb_batch_verifier) sums these checks with random weights over
+// any number of proofs and circuits: one shared g-term, one variable-base MSM per call.
 #define TB_NOINLINE_MUL 1
 #include <algorithm>
 #include <cstdlib>
@@ -58,15 +58,6 @@ struct VTranscript : Transcript {
   }
 };
 
-// out[k][t] = -(c_k * s_t),  s_t = prod_j u_{k,j}^{bit_(kk-1-j)(t)};  t = 0 additionally gets -v_k
-__global__ void verify_g_scalars_kernel(const Fp* __restrict__ us, const Fp* __restrict__ cv, Fp* __restrict__ out, int kk, int n) {
-  int t = blockIdx.x * blockDim.x + threadIdx.x, p = blockIdx.y;
-  if (t >= n) return;
-  Fp s = cv[2 * p];
-  for (int j = 0; j < kk; ++j) if ((t >> (kk - 1 - j)) & 1) s = s * us[(size_t)p * kk + j];
-  if (t == 0) s = s + cv[2 * p + 1];
-  st_fe(out + (size_t)p * n + t, s.neg());
-}
 __global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_t* ok, int K) {
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= K) return;
@@ -74,74 +65,67 @@ __global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_
   ok[p] = s.is_inf() ? 1 : 0;
 }
 
-// the proof's evaluations at x, as argument.cuh reads them
+// the proof's evaluations at x (C.evals order, then the expected h(x)), as argument.cuh reads them
 struct EvalView {
-  const Shape& C; std::map<std::pair<PolyId, int>, Fp>& ev; int last_rot;
-  Fp perm_col(int c) const { const tb_column& col = C.perm[c]; return ev[{{col.kind == TB_COL_ADVICE ? PK_ADV : col.kind == TB_COL_FIXED ? PK_FIXED : PK_INST, (int)col.index}, 0}]; }
-  Fp sigma(int c) const { return ev[{{PK_SIG, c}, 0}]; }
-  Fp z(int s) const { return ev[{{PK_PZ, s}, 0}]; }
-  Fp z_next(int s) const { return ev[{{PK_PZ, s}, 1}]; }
-  Fp z_last(int s) const { return ev[{{PK_PZ, s}, last_rot}]; }
+  const Shape& C; const std::vector<Fp>& ev; int last_rot;
+  Fp at(const PolyId& poly, int rot) const { return ev[C.eval_index(poly, rot)]; }
+  Fp perm_col(int c) const { return at(column_poly(C.perm[c]), 0); }
+  Fp sigma(int c) const { return at({PK_SIG, c}, 0); }
+  Fp z(int s) const { return at({PK_PZ, s}, 0); }
+  Fp z_next(int s) const { return at({PK_PZ, s}, 1); }
+  Fp z_last(int s) const { return at({PK_PZ, s}, last_rot); }
 };
 
-// sum(instance_len); refuses an instance column longer than the usable rows (InstanceTooLarge)
-static size_t instance_total(const Shape& C, const uint32_t* instance_len) {
-  size_t total = 0;
-  for (uint32_t c = 0; c < C.ni; ++c) { TB_REQUIRE(instance_len[c] <= C.usable, "InstanceTooLarge"); total += instance_len[c]; }
-  return total;
+// commit_lagrange(column, Blind::default()) of `count` columns of n values at `vals` ([count][n], Montgomery): the points,
+// Montgomery, on the host
+static std::vector<Aff<Fq>> commit_columns(Ctx* ctx, const Srs& srs, const Fp* vals, int count) {
+  std::vector<Aff<Fq>> out(count, Aff<Fq>::inf());
+  if (!count) return out;
+  DevBuf<Fp> ones(ctx, count); DevBuf<Aff<Fq>> pts(ctx, count);
+  std::vector<Fp> h(count, Fp::one()); ones.upload(h.data(), count);
+  srs.commit(ctx, true, vals, (long long)srs.n, count, ones.get(), pts.get());
+  pts.download(out.data(), count); ctx->sync();
+  return out;
 }
 
-// What the transcript replay of K proofs leaves for their final IPA checks.  Proof p's variable-base terms are pts / sc at
-// [p * stride, p * stride + M), unused slots the identity times 0.  With `wu_terms` the last two of them are W and U with
-// their scalars -f and -c*b*z and stride = M; otherwise stride is M rounded up to a power of two.  extras[p] = (-f, -c*b*z)
-// either way, us[p] = the kk IPA challenges u_j, cv[p] = (c, v).  alive[p] = 0 for a proof rejected during the replay (a read
-// that fails, an identity absorbed, a non-canonical scalar or instance value, trailing bytes); its terms are all unused.
+// What the transcript replay of K proofs leaves for their final IPA checks.  Proof p's M variable-base terms are pts / sc at
+// [p * M, (p + 1) * M), the last two W and U with their scalars -f and -c*b*z; us[p] = the kk IPA challenges u_j and
+// ab[p] = (-c, -v), the coefficients of its g-term.  alive[p] = 0 for a proof rejected during the replay (a read that fails,
+// an identity absorbed, a non-canonical scalar or instance value, trailing bytes); its terms are the identity times 0, its ab 0.
 struct Replay {
-  int M = 0, stride = 0;
-  std::vector<Aff<Fq>> pts; std::vector<Fp> sc, us, cv, extras; std::vector<char> alive;
+  int M = 0;
+  std::vector<Aff<Fq>> pts; std::vector<Fp> sc, us, ab; std::vector<char> alive;
 };
 
 // Replays the transcripts of K proofs of proof_len == C.proof_len bytes of the circuit of shape C, whose fixed / sigma
 // commitments are `vk_fixed` / `vk_sigma` (Montgomery).  Every point is decoded and every instance column committed on the
 // device first.
 static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
-                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len,
-                         bool wu_terms, Replay& rep) {
-  const size_t n = C.n; const int kk = (int)C.k, na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf, nf = C.nf, pieces = C.pieces;
-  cudaStream_t st = ctx->stream;
+                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, Replay& rep) {
+  const size_t n = C.n; const int kk = (int)C.k, na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf, pieces = C.pieces;
   const size_t inst_total = instance_total(C, instance_len);
   // ---- every point of the batch, decoded on the device: [K][npts]
   const int npts = (int)C.point_offsets.size();
   std::vector<Aff<Fq>> dec((size_t)K * npts);
   std::vector<uint8_t> dec_ok((size_t)K * npts);
   { DevBuf<uint8_t> d_proofs(ctx, (size_t)K * proof_len), d_ok(ctx, dec_ok.size()); DevBuf<uint32_t> d_off(ctx, npts); DevBuf<Aff<Fq>> d_pts(ctx, dec.size());
-    TB_CUDA(cudaMemcpy2DAsync(d_proofs.get(), proof_len, proofs, proof_stride, proof_len, K, cudaMemcpyHostToDevice, st));
+    TB_CUDA(cudaMemcpy2DAsync(d_proofs.get(), proof_len, proofs, proof_stride, proof_len, K, cudaMemcpyHostToDevice, ctx->stream));
     d_off.upload(C.point_offsets.data(), npts);
     decompress(ctx, d_proofs.get(), proof_len, d_off.get(), npts, dec.size(), d_pts.get(), d_ok.get());
     d_pts.download(dec.data(), dec.size()); d_ok.download(dec_ok.data(), dec_ok.size()); ctx->sync(); }
-  // ---- instance commitments for the whole batch: commit_lagrange(instance, Blind::default())
-  std::vector<Aff<Fq>> inst_comm((size_t)K * std::max(1, ni), Aff<Fq>::inf());
+  // ---- instance commitments for the whole batch: [K][ni]
+  std::vector<Aff<Fq>> inst_comm;
   if (ni) {
-    DevBuf<Fp> iv(ctx, (size_t)K * ni * n), ones(ctx, (size_t)K * ni); DevBuf<Aff<Fq>> pts(ctx, (size_t)K * ni);
-    iv.zero();
-    size_t off = 0;
-    for (int c = 0; c < ni; ++c) {
-      if (instance_len[c])
-        TB_CUDA(cudaMemcpy2DAsync(iv.get() + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, K, cudaMemcpyHostToDevice, st));
-      off += instance_len[c];
-    }
-    fe_to_mont<Fp>(ctx, iv.get(), (size_t)K * ni * n);
-    std::vector<Fp> h((size_t)K * ni, Fp::one()); ones.upload(h.data(), h.size());
-    srs.commit(ctx, true, iv.get(), (long long)n, K * ni, ones.get(), pts.get());
-    pts.download(inst_comm.data(), (size_t)K * ni); ctx->sync();
+    DevBuf<Fp> iv(ctx, (size_t)K * ni * n);
+    upload_instance(ctx, C, K, instance, instance_len, iv.get());
+    inst_comm = commit_columns(ctx, srs, iv.get(), K * ni);
   }
   // ---- per proof: replay the transcript, accumulate (scalar, point) pairs
   const int nps = (int)C.point_sets.size();
-  rep.M = ni + na + 3 * L + nsets + 1 + pieces + nf + P + 2 + 2 * kk + (wu_terms ? 2 : 0);   // variable-base terms per proof
-  if (wu_terms) rep.stride = rep.M;
-  else { rep.stride = 32; while (rep.stride < rep.M) rep.stride *= 2; }
-  rep.pts.assign((size_t)K * rep.stride, Aff<Fq>::inf());
-  rep.sc.assign((size_t)K * rep.stride, Fp::zero()); rep.us.assign((size_t)K * kk, Fp::zero()); rep.cv.assign((size_t)K * 2, Fp::zero()); rep.extras.assign((size_t)K * 2, Fp::zero());
+  // variable-base terms per proof: every committed polynomial (h in its pieces), q', S, the L_j and R_j, W and U
+  rep.M = (int)C.uniq.size() - 1 + pieces + 2 + 2 * kk + 2;
+  rep.pts.assign((size_t)K * rep.M, Aff<Fq>::inf());
+  rep.sc.assign((size_t)K * rep.M, Fp::zero()); rep.us.assign((size_t)K * kk, Fp::zero()); rep.ab.assign((size_t)K * 2, Fp::zero());
   rep.alive.assign(K, 0);
   const Fp one = Fp::one();
   const int last_rot = -(bf + 1);
@@ -169,13 +153,11 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     for (int i = 0; i < pieces && ok; ++i) ok = tr.read_point(hpts[i]);
     Fp x = tr.squeeze();
     if (!ok) continue;
-    // evaluations, in the prover's order (C.evals)
-    std::map<std::pair<PolyId, int>, Fp> ev;
-    for (auto& e : C.evals) {
-      Fp v; if (!tr.read_scalar(v)) { ok = false; break; }
-      ev[{e.poly, e.rot}] = v;
-    }
+    // evaluations, in the prover's order (C.evals); the last entry is set to the expected h(x) below
+    std::vector<Fp> ev(C.evals.size() + 1, Fp::zero());
+    for (size_t i = 0; i < C.evals.size() && ok; ++i) ok = tr.read_scalar(ev[i]);
     if (!ok) continue;
+    const EvalView view{C, ev, last_rot};
     // expected h(x)
     Fp xn = x; for (int i = 0; i < kk; ++i) xn = xn.sqr();
     auto l_at = [&](int rot) { Fp wi = rot_pow(rot); return (xn - one) * n_inv * wi * (x - wi).inv(); };
@@ -185,17 +167,18 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     const int J = (int)C.plan.num_constraints;
     std::vector<Fp> ypow(J + C.plan.t_pl + 2, one), lk_a(L), lk_t(L);
     for (size_t i = 1; i < ypow.size(); ++i) ypow[i] = ypow[i - 1] * y;
-    auto at_x = [&](int kind, int col, int rot) { return ev[{{kind == K_ADV ? PK_ADV : kind == K_FIX ? PK_FIXED : PK_INST, col}, rot}]; };
+    auto at_x = [&](int kind, int col, int rot) { return view.at({kind == K_ADV ? PK_ADV : kind == K_FIX ? PK_FIXED : PK_INST, col}, rot); };
     PointMachine<decltype(at_x)> m{at_x, C.consts_host.data(), ypow.data(), theta, lk_a.data(), lk_t.data()};
     Fp acc = Fp::zero();
     for (const auto* parts : {&C.plan.gate_parts[0], &C.plan.gate_parts_lo[0]})
       for (const GateProgram& g : *parts) acc = acc + ypow[J - 1 - g.last] * m.run(g);
     m.run(C.plan.lookups);
     const ArgPoint at = {y, beta, gamma, l_0, l_last, one - (l_last + l_blind)};
-    acc = perm_fold(acc, EvalView{C, ev, last_rot}, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
+    acc = perm_fold(acc, view, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
     for (int l = 0; l < L; ++l)
-      acc = lookup_fold(acc, at, ev[{{PK_LZ, l}, 0}], ev[{{PK_LZ, l}, 1}], ev[{{PK_LPIN, l}, 0}], ev[{{PK_LPIN, l}, -1}], ev[{{PK_LPTAB, l}, 0}], lk_a[l], lk_t[l]);
-    ev[{{PK_H, 0}, 0}] = acc * (xn - one).inv();
+      acc = lookup_fold(acc, at, view.at({PK_LZ, l}, 0), view.at({PK_LZ, l}, 1), view.at({PK_LPIN, l}, 0), view.at({PK_LPIN, l}, -1), view.at({PK_LPTAB, l}, 0),
+                        lk_a[l], lk_t[l]);
+    ev[C.eval_index({PK_H, 0}, 0)] = acc * (xn - one).inv();
     // ---- multiopen
     Fp x1 = tr.squeeze(), x2 = tr.squeeze();
     std::vector<std::vector<Fp>> q_evals(nps);
@@ -206,11 +189,7 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
       for (int c = (int)C.uniq.size() - 1; c >= 0; --c) { int s = C.uniq_set[c]; coef_in_set[C.uniq[c]] = cur[s]; cur[s] = cur[s] * x1; }
       for (size_t c = 0; c < C.uniq.size(); ++c) {
         int s = C.uniq_set[c];
-        for (size_t pi = 0; pi < C.point_sets[s].size(); ++pi) {
-          auto it = ev.find({C.uniq[c], C.point_sets[s][pi]});
-          if (it == ev.end()) { ok = false; break; }
-          q_evals[s][pi] = q_evals[s][pi] * x1 + it->second;
-        }
+        for (size_t pi = 0; pi < C.point_sets[s].size(); ++pi) q_evals[s][pi] = q_evals[s][pi] * x1 + view.at(C.uniq[c], C.point_sets[s][pi]);
       } }
     Aff<Fq> q_prime; ok = ok && tr.read_point(q_prime);
     Fp x3 = tr.squeeze();
@@ -239,7 +218,7 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     if (!ok || tr.bad || tr.pos != proof_len) continue;
     Fp b = one; { Fp cur = x3; for (int j = kk - 1; j >= 0; --j) { b = b * (one + uj[j] * cur); cur = cur * cur; } }
     // ---- variable-base terms
-    Aff<Fq>* pp = rep.pts.data() + (size_t)p * rep.stride; Fp* ss = rep.sc.data() + (size_t)p * rep.stride; int w = 0;
+    Aff<Fq>* pp = rep.pts.data() + (size_t)p * rep.M; Fp* ss = rep.sc.data() + (size_t)p * rep.M; int w = 0;
     auto push = [&](const Aff<Fq>& pt, const Fp& sc) { pp[w] = pt; ss[w] = sc; ++w; };
     for (size_t c = 0; c < C.uniq.size(); ++c) {
       const PolyId& id = C.uniq[c]; Fp coef = coef_in_set[id] * x4pow[nps - 1 - C.uniq_set[c]];
@@ -251,35 +230,32 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
     push(q_prime, x4pow[nps]);
     push(s_comm, xi);
     for (int j = 0; j < kk; ++j) { push(Ls[j], uj[j].inv()); push(Rs[j], uj[j]); }
-    rep.extras[2 * p] = ff.neg();                    // * W
-    rep.extras[2 * p + 1] = (cc * b * z).neg();      // * U
-    if (wu_terms) { push(srs.w_host, rep.extras[2 * p]); push(srs.u_host, rep.extras[2 * p + 1]); }
-    if (w > rep.stride) throw std::runtime_error("internal error: verifier term count");
+    push(srs.w_host, ff.neg());
+    push(srs.u_host, (cc * b * z).neg());
+    if (w != rep.M) throw std::logic_error("internal error: verifier term count");
     for (int j = 0; j < kk; ++j) rep.us[(size_t)p * kk + j] = uj[j];
-    rep.cv[2 * p] = cc; rep.cv[2 * p + 1] = v;
+    rep.ab[2 * p] = cc.neg(); rep.ab[2 * p + 1] = v.neg();
     rep.alive[p] = 1;
   }
 }
 
 // n_proofs proofs of the circuit of shape C, each checked on its own: the replay, then both MSMs of every proof's final
-// check for the whole batch on the device, then the identity test
+// check for the whole batch on the device (each proof its own g-term), then the identity test
 static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
                          const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
-  const size_t n = C.n; const int kk = (int)C.k;
+  const size_t n = C.n;
   instance_total(C, instance_len);
   for (int p = 0; p < K; ++p) ok_out[p] = 0;
   if (proof_len != C.proof_len) return;   // no proof of this length is accepted
   Replay r;
-  replay_batch(ctx, C, srs, vk_fixed, vk_sigma, K, instance, instance_len, proofs, proof_stride, proof_len, false, r);
-  const int Mpad = r.stride;
-  DevBuf<Aff<Fq>> d_pts(ctx, r.pts.size()); DevBuf<Fp> d_sc(ctx, r.sc.size()), d_us(ctx, r.us.size()), d_cv(ctx, r.cv.size()), d_ex(ctx, r.extras.size()), d_gs(ctx, (size_t)K * n);
+  replay_batch(ctx, C, srs, vk_fixed, vk_sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r);
+  DevBuf<Aff<Fq>> d_pts(ctx, r.pts.size()); DevBuf<Fp> d_sc(ctx, r.sc.size()), d_us(ctx, r.us.size()), d_ab(ctx, r.ab.size()), d_gs(ctx, (size_t)K * n);
   DevBuf<Xyzz<Fq>> acc_v(ctx, K), acc_g(ctx, K); DevBuf<uint8_t> d_ok(ctx, K);
-  d_pts.upload(r.pts.data(), r.pts.size()); d_sc.upload(r.sc.data(), r.sc.size()); d_us.upload(r.us.data(), r.us.size()); d_cv.upload(r.cv.data(), r.cv.size());
-  d_ex.upload(r.extras.data(), r.extras.size());
-  MsmConfig cfg;
-  msm_run<Fq, Fp>(ctx, d_sc.get(), (long long)Mpad, d_pts.get(), (long long)Mpad, Mpad, K, cfg, acc_v.get());
-  launch(ctx, verify_g_scalars_kernel, dim3((unsigned)((n + 255) / 256), K), 256, 0, d_us.get(), d_cv.get(), d_gs.get(), kk, (int)n);
-  srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, d_ex.get(), 2, acc_g.get());
+  d_pts.upload(r.pts.data(), r.pts.size()); d_sc.upload(r.sc.data(), r.sc.size()); d_us.upload(r.us.data(), r.us.size()); d_ab.upload(r.ab.data(), r.ab.size());
+  d_gs.zero();
+  msm_run<Fq, Fp>(ctx, d_sc.get(), r.M, d_pts.get(), r.M, r.M, K, MsmConfig(), acc_v.get());
+  batch_g_scalars(ctx, d_gs.get(), d_us.get(), d_ab.get(), (int)C.k, K, 1);
+  srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
   launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K);
   std::vector<uint8_t> hok(K);
   d_ok.download(hok.data(), K); ctx->sync();
@@ -301,12 +277,11 @@ struct BatchVerifier {
   DevMem<Xyzz<Fq>> acc;     // [1] sum_p rho_p (every variable-base term of proof p, W and U included)
 };
 
-// Per proof p of a call (one CTA each): its M variable-base scalars times rho_p, and ab[p] = (-rho_p c_p, -rho_p v_p), the
-// coefficients of its g-term.
-__global__ void batch_weights_kernel(const Fp* __restrict__ rho, Fp* __restrict__ sc, int M, const Fp* __restrict__ cv, Fp* __restrict__ ab) {
+// Per proof p of a call (one CTA each): its M variable-base scalars and ab[p], the coefficients of its g-term, times rho_p
+__global__ void batch_weights_kernel(const Fp* __restrict__ rho, Fp* __restrict__ sc, int M, Fp* __restrict__ ab) {
   const int p = blockIdx.x;
   const Fp w = ldg_fe(rho + p);
-  if (threadIdx.x < 2) st_fe(ab + 2 * p + threadIdx.x, (w * ldg_fe(cv + 2 * p + threadIdx.x)).neg());
+  if (threadIdx.x < 2) { Fp* a = ab + 2 * p + threadIdx.x; st_fe(a, ld_fe(a) * w); }
   for (int i = threadIdx.x; i < M; i += blockDim.x) { Fp* s = sc + (size_t)p * M + i; st_fe(s, ld_fe(s) * w); }
 }
 
@@ -314,19 +289,22 @@ __global__ void batch_acc_kernel(Xyzz<Fq>* acc, const Xyzz<Fq>* add) {
   Xyzz<Fq> s = *acc; s.add(*add); *acc = s;
 }
 
-// G[t] += sum_p (a_p s_{p,t} + [t = 0] b_p), s_{p,t} = prod_j u_{p,j}^{bit_(kk-1-j)(t)}, (a_p, b_p) = ab[p].  With t = hi * 2^lb
-// + lo (lb = min(kk, BG_LOG)), s_{p,t} = H_p(hi) * L_p(lo), H over the top kk - lb bits, L over the low lb bits.  One CTA per
-// hi: for BG_PROOFS proofs at a time it writes a_p H_p(hi) into entry 0 of a table in shared memory and doubles the table lb
-// times (entries [m, 2m) = entries [0, m) times the u of bit log2(m)), which leaves a_p s_{p,t} in entry lo; each thread then
-// adds its entries.  One product per (proof, t), plus ~(kk - lb)/2 per (proof, CTA) for H.
+// G[g][t] += sum_{p in group g} (a_p s_{p,t} + [t = 0] b_p), s_{p,t} = prod_j u_{p,j}^{bit_(kk-1-j)(t)}, (a_p, b_p) = ab[p],
+// group g = proofs [g * group, min((g + 1) * group, K)).  With t = hi * 2^lb + lo (lb = min(kk, BG_LOG)), s_{p,t} = H_p(hi) *
+// L_p(lo), H over the top kk - lb bits, L over the low lb bits.  One CTA per (hi, g): for BG_PROOFS proofs at a time it writes
+// a_p H_p(hi) into entry 0 of a table in shared memory and doubles the table lb times (entries [m, 2m) = entries [0, m) times
+// the u of bit log2(m)), which leaves a_p s_{p,t} in entry lo; each thread then adds its entries.  One product per (proof, t),
+// plus ~(kk - lb)/2 per (proof, CTA) for H.
 constexpr int BG_LOG = 8, BG_THREADS = 1 << BG_LOG, BG_PROOFS = 4;
-__global__ void __launch_bounds__(BG_THREADS) batch_g_scalars_kernel(Fp* __restrict__ G, const Fp* __restrict__ us, const Fp* __restrict__ ab, int kk, int K) {
+__global__ void __launch_bounds__(BG_THREADS) batch_g_scalars_kernel(Fp* __restrict__ G, const Fp* __restrict__ us, const Fp* __restrict__ ab, int kk, int K,
+                                                                     int group) {
   __shared__ Fp tab[BG_PROOFS][BG_THREADS];
   const int lb = kk < BG_LOG ? kk : BG_LOG, lo = threadIdx.x;
   const uint32_t hi = blockIdx.x;
+  const int p_end = min(K, (int)(blockIdx.y + 1) * group);
   Fp acc = Fp::zero();
-  for (int p0 = 0; p0 < K; p0 += BG_PROOFS) {
-    const int np = K - p0 < BG_PROOFS ? K - p0 : BG_PROOFS;
+  for (int p0 = blockIdx.y * group; p0 < p_end; p0 += BG_PROOFS) {
+    const int np = p_end - p0 < BG_PROOFS ? p_end - p0 : BG_PROOFS;
     if (lo < np) {
       const Fp* u = us + (size_t)(p0 + lo) * kk;
       Fp h = ldg_fe(ab + 2 * (p0 + lo));
@@ -345,15 +323,15 @@ __global__ void __launch_bounds__(BG_THREADS) batch_g_scalars_kernel(Fp* __restr
     if (hi == 0 && lo == 0) for (int q = 0; q < np; ++q) acc = acc + ldg_fe(ab + 2 * (p0 + q) + 1);
     __syncthreads();
   }
-  if (lo < (1 << lb)) { Fp* g = G + ((size_t)hi << lb) + lo; st_fe(g, ld_fe(g) + acc); }
+  if (lo < (1 << lb)) { Fp* g = G + ((size_t)blockIdx.y << kk) + ((size_t)hi << lb) + lo; st_fe(g, ld_fe(g) + acc); }
 }
 
-void batch_g_scalars(Ctx* ctx, Fp* G, const Fp* us, const Fp* ab, int kk, int K) {
-  TB_REQUIRE(kk >= 1 && kk <= 30 && K >= 1, "batch_g_scalars shape");
+void batch_g_scalars(Ctx* ctx, Fp* G, const Fp* us, const Fp* ab, int kk, int K, int group) {
+  TB_REQUIRE(kk >= 1 && kk <= 30 && K >= 1 && group >= 1 && (K - 1) / group < 65535, "batch_g_scalars shape");
   const int lb = kk < BG_LOG ? kk : BG_LOG;
   ProfScope scope(ctx, PC_IPA_FOLD);
   ctx->work[PC_IPA_FOLD] += (double)K * (double)(1ull << kk) * (1.0 + 0.5 * (kk - lb) / (1 << lb));
-  launch(ctx, batch_g_scalars_kernel, (unsigned)(1u << (kk - lb)), BG_THREADS, 0, G, us, ab, kk, K);
+  launch(ctx, batch_g_scalars_kernel, dim3(1u << (kk - lb), (unsigned)((K - 1) / group + 1)), BG_THREADS, 0, G, us, ab, kk, K, group);
 }
 
 // The proofs of one tb_batch_verifier_add: replay, then (unless a proof was rejected) their weights, their terms through one
@@ -365,22 +343,22 @@ static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K
   if (!bv.rejected && proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted
   if (!bv.rejected) {
     Replay r;
-    replay_batch(ctx, C, *vk.srs, vk.fixed, vk.sigma, K, instance, instance_len, proofs, proof_stride, proof_len, true, r);
+    replay_batch(ctx, C, *vk.srs, vk.fixed, vk.sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r);
     if (std::find(r.alive.begin(), r.alive.end(), 0) != r.alive.end()) bv.rejected = true;
     else {
       const size_t N = (size_t)K * r.M;
-      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_cv(ctx, r.cv.size()), d_rho(ctx, K), d_ab(ctx, 2 * (size_t)K);
+      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_rho(ctx, K), d_ab(ctx, r.ab.size());
       DevBuf<Xyzz<Fq>> part(ctx, 1);
-      d_pts.upload(r.pts.data(), N); d_sc.upload(r.sc.data(), N); d_us.upload(r.us.data(), r.us.size()); d_cv.upload(r.cv.data(), r.cv.size());
+      d_pts.upload(r.pts.data(), N); d_sc.upload(r.sc.data(), N); d_us.upload(r.us.data(), r.us.size()); d_ab.upload(r.ab.data(), r.ab.size());
       bv.broken = true;
       { ProfScope scope(ctx, PC_IPA_FOLD);
         prf_fill(ctx, bv.seed, j0, R_BATCH_WEIGHT, 0, d_rho.get(), 1, 1, 1, K);
         ctx->work[PC_IPA_FOLD] += (double)K * (r.M + 2);
-        launch(ctx, batch_weights_kernel, K, 128, 0, d_rho.get(), d_sc.get(), r.M, d_cv.get(), d_ab.get()); }
+        launch(ctx, batch_weights_kernel, K, 128, 0, d_rho.get(), d_sc.get(), r.M, d_ab.get()); }
       msm_run<Fq, Fp>(ctx, d_sc.get(), 0, d_pts.get(), 0, (int)N, 1, MsmConfig(), part.get());
       { ProfScope scope(ctx, PC_MSM_REDUCE);
         launch(ctx, batch_acc_kernel, 1, 1, 0, bv.acc.get(), part.get()); }
-      batch_g_scalars(ctx, bv.g.get(), d_us.get(), d_ab.get(), (int)C.k, K);
+      batch_g_scalars(ctx, bv.g.get(), d_us.get(), d_ab.get(), (int)C.k, K, K);
       ctx->sync();   // the batch may be used from another context (stream) next
       bv.broken = false;
     }
@@ -403,18 +381,15 @@ static uint8_t batch_finalize(Ctx* ctx, const BatchVerifier& bv) {
 static const Circuit& pk_commitments(Ctx* ctx, const Circuit& C) {
   std::lock_guard<std::mutex> vk_lock(C.mu);
   if (C.vk_fixed.size() != (size_t)C.nf || C.vk_sigma.size() != (size_t)C.P) {
-    for (int which = 0; which < 2; ++which) {
-      int cnt = which ? (int)C.P : (int)C.nf;
-      std::vector<Aff<Fq>>& dst = which ? C.vk_sigma : C.vk_fixed;
-      dst.assign(cnt, Aff<Fq>::inf());
-      if (!cnt) continue;
-      DevBuf<Fp> ones(ctx, cnt); DevBuf<Aff<Fq>> pts(ctx, cnt);
-      std::vector<Fp> h(cnt, Fp::one()); ones.upload(h.data(), cnt);
-      C.srs->commit(ctx, true, which ? C.sig_vals.get() : C.fixed_vals.get(), (long long)C.n, cnt, ones.get(), pts.get());
-      pts.download(dst.data(), cnt); ctx->sync();
-    }
+    C.vk_fixed = commit_columns(ctx, *C.srs, C.fixed_vals.get(), (int)C.nf);
+    C.vk_sigma = commit_columns(ctx, *C.srs, C.sig_vals.get(), (int)C.P);
   }
   return C;
+}
+
+// Montgomery points -> 64 bytes each: canonical affine x || y, 64 zero bytes = the identity (the inverse of parse_commitments)
+static void store_commitments(const std::vector<Aff<Fq>>& pts, uint8_t* b) {
+  for (const Aff<Fq>& p : pts) { Aff<Fq> c = p.from_mont(); memcpy(b, c.x.l, 32); memcpy(b + 32, c.y.l, 32); b += 64; }
 }
 
 // cnt commitments of 64 bytes (canonical affine x || y, 64 zero bytes = the identity) -> Montgomery points; refuses a
@@ -445,6 +420,18 @@ tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const
   TB_CUDA(cudaSetDevice(ctx->c.device));
   pk_commitments(&ctx->c, *C);
   verify_batch(&ctx->c, *C, *C->srs, C->vk_fixed, C->vk_sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
+  TB_API_END(ctx)
+}
+
+// keygen_vk on the device: commit_lagrange(column, Blind::default() = 1) of every fixed and sigma column
+tb_status tb_pk_commitments(tb_ctx* ctx, const tb_pk* pk, uint8_t* fixed_commitments, uint8_t* sigma_commitments) {
+  TB_API_BEGIN(ctx)
+  const Circuit* C = reinterpret_cast<const Circuit*>(pk);
+  TB_REQUIRE(C && (fixed_commitments || C->nf == 0) && (sigma_commitments || C->P == 0), "tb_pk_commitments arguments");
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  pk_commitments(&ctx->c, *C);
+  store_commitments(C->vk_fixed, fixed_commitments);
+  store_commitments(C->vk_sigma, sigma_commitments);
   TB_API_END(ctx)
 }
 

@@ -11,7 +11,8 @@ proofs of any circuits over one SRS, from the random-weighted sum of their final
   unweighted sum would accept; the batch rejects it in one call, across two calls and across the two Taiga circuits, under
   three seeds.
 * More than one call's limit (4160 proofs), refusals that leave the batch as it was, and ProverService.verify_ptx_batch.
-* The g-term kernel on its own through the test probe, against a Python big-integer sum."""
+* The g-term kernel on its own through the test probe, against a Python big-integer sum, with all proofs in one group (the
+  batch verifier) and with one proof per group (the per-proof verifier)."""
 import ctypes
 import os
 import random
@@ -386,3 +387,15 @@ def test_g_scalars_kernel(gpu_ctx, k, K):
         want = g_ref(want, us, ab, k)
         expect("batch_g_scalars k=%d K=%d, call %d" % (k, K, call), probe.get(d_G), want)
         assert probe.get(d_us) == [x for u in us for x in u]
+    # the same driver with one proof per group (the per-proof verifier): proof p's terms added into row p of [K][n] alone
+    so.tbp_batch_g_scalars_grouped.restype = ctypes.c_int
+    so.tbp_batch_g_scalars_grouped.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3
+    rows = [[rnd.randrange(P) for _ in range(n)] for _ in range(K)]
+    d_rows = probe.put([x for r in rows for x in r])
+    us = [[field() for _ in range(k)] for _ in range(K)]
+    ab = [(field(), field()) for _ in range(K)]
+    d_us, d_ab = probe.put([x for u in us for x in u]), probe.put([x for p in ab for x in p])
+    probe.run("tbp_batch_g_scalars_grouped", addr(d_rows), addr(d_us), addr(d_ab), k, K, 1)
+    got = probe.get(d_rows)
+    for p in range(K):
+        expect("batch_g_scalars k=%d K=%d, one proof per group, proof %d" % (k, K, p), got[p * n:(p + 1) * n], g_ref(rows[p], us[p:p + 1], ab[p:p + 1], k))

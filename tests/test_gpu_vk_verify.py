@@ -9,7 +9,8 @@
   and a proof's verdict does not depend on the rest of its batch.
 * A vk made of the proving key's commitments, kept as bytes, verifies on a fresh context after the key and its context
   are gone; a vk with two fixed commitments swapped, one sigma commitment replaced or another transcript representation
-  rejects every proof; malformed commitments and descriptions are refused and the context keeps working."""
+  rejects every proof; malformed commitments and descriptions (among them an equality-enabled column without its
+  rotation-0 query) are refused and the context keeps working."""
 import copy
 import ctypes
 import os
@@ -25,7 +26,7 @@ from taiga_b200 import circuits_mini as cm
 from taiga_b200 import circuits_random as cr
 from taiga_b200 import circuits_taiga as ct
 from taiga_b200 import lib
-from taiga_b200.circuit import TbCsDesc
+from taiga_b200.circuit import TbCsDesc, TbQuery
 
 from test_gpu_verifier_soundness import PROVE_SHAPES, stack
 from test_verifier_soundness import MUTANT_SHAPES, SEED, References, mutant_shape
@@ -375,4 +376,30 @@ def test_refused_loads_leave_the_context_usable(srs_for):
         vk = gsrs.load_verifying_key(kd, f, s)
         assert vk.verify_batch(inst, lens, proofs) == [True, True], what
         vk.close()
+    pk.close()
+
+
+def test_permutation_column_without_rotation_0_query_refused(srs_for):
+    """halo2's enable_equality queries the column at rotation 0, and the permutation argument reads the column there: a
+    descriptor that moves that query to another rotation is refused by both loads, naming the column."""
+    kd, make = cm.standard_plonk(k=6, n_lookups=2)
+    _, gsrs = srs_for(6)
+    pk = gsrs.load_circuit(kd)
+    proofs, inst, lens = _honest(kd, make, pk, 2)
+    f, s = pk.commitments()
+    col = kd.desc.perm_columns[0]
+    field = ("advice", "fixed", "instance")[col.kind] + "_queries"
+    qs = [(q.column, q.rotation) for q in getattr(kd.desc, field)[:getattr(kd.desc, "num_" + field)]]
+    i = qs.index((col.index, 0))
+    rot = max(r for c, r in qs if c == col.index) + 1     # a rotation the column has no other query at
+    moved = (TbQuery * len(qs))(*[TbQuery(c, rot if j == i else r) for j, (c, r) in enumerate(qs)])
+    bad = _with_desc(kd, **{field: moved})
+    bad.moved_queries = moved
+    for what, load in (("load_verifying_key", lambda: gsrs.load_verifying_key(bad, f, s)), ("load_circuit", lambda: gsrs.load_circuit(bad))):
+        with pytest.raises(lib.TaigaB200Error) as e:
+            load()
+        assert e.value.status == lib.TB_ERR_INVALID and "permutation column 0 (" in str(e.value) and "has no rotation-0 query" in str(e.value), (what, str(e.value))
+    vk = gsrs.load_verifying_key(kd, f, s)
+    assert both(pk, vk, inst, lens, proofs) == [True, True]
+    vk.close()
     pk.close()
