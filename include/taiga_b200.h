@@ -30,6 +30,8 @@ enum { TB_VESTA = 0, TB_PALLAS = 1 };
 
 typedef struct tb_ctx tb_ctx;
 typedef struct tb_srs tb_srs;
+typedef struct tb_vk tb_vk;                          /* verifying key (below) */
+typedef struct tb_batch_verifier tb_batch_verifier;  /* batch verifier (below) */
 
 /* ---- context (owns a CUDA stream, twiddle tables, stream-ordered scratch memory) */
 tb_status tb_ctx_create(int device, tb_ctx** out);
@@ -74,6 +76,21 @@ tb_status tb_dev_ntt(tb_ctx* ctx, int field, uint32_t logn, int inverse, int cos
                      void* d_scratch /* batch << logn elements; may alias d_in if the input may be destroyed */);
 tb_status tb_dev_msm(tb_ctx* ctx, int curve, size_t n, uint32_t batch, const void* d_scalars, const void* d_points,
                      uint32_t window_bits, void* d_out_points /* batch affine points, Montgomery */);
+/* Verification of proofs that are already in device memory (proofs gathered from other GPUs, proofs this process made):
+ * tb_verify_batch_vk and tb_batch_verifier_add (below) with d_instance, d_proofs and d_ok_out in device memory of the
+ * context's device, in the layouts and encodings of the host versions (canonical bytes, not Montgomery residues);
+ * instance_len is a host array.  Any proof_stride >= proof_len is allowed, odd ones included.  The transcripts are replayed
+ * on the device, one thread per proof, and the call enqueues all its work on the context's stream and returns without
+ * waiting: d_ok_out[i] (1 or 0) is written in stream order, and the caller keeps every buffer alive and unmodified until the
+ * stream has passed the call.  Each call refuses (TB_ERR_INVALID, nothing enqueued) what its host version refuses, and a
+ * buffer that is not device memory of the context's device.  Verdicts are those of tb_verify_batch_vk on the same bytes; a
+ * proof_len other than tb_vk_proof_len gives 0 for every proof.  Device and host adds mix freely in one batch (j counts
+ * across both); a proof a device add rejects makes finalize give 0, which finalize learns in its one download, so finalize
+ * stays the batch's only wait.  A batch moved to another context after a device add first waits for the device. */
+tb_status tb_dev_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk, uint32_t n_proofs, const void* d_instance, const uint32_t* instance_len,
+                                 const void* d_proofs, size_t proof_stride, size_t proof_len, void* d_ok_out);
+tb_status tb_dev_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv, const tb_vk* vk, uint32_t n_proofs, const void* d_instance,
+                                    const uint32_t* instance_len, const void* d_proofs, size_t proof_stride, size_t proof_len);
 
 /* ---- circuit description.  Replaces what halo2_proofs keeps inside ProvingKey<vesta::Affine> / VerifyingKey.cs
  * (COMPLIANCE_PROVING_KEY, taiga_halo2/src/constant.rs:145-152; TRIVIAL_RESOURCE_LOGIC_PK,
@@ -187,7 +204,6 @@ tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const
  * commitment with a coordinate >= q or off the curve.  A tb_vk holds host memory only (no per-row table) and refers to
  * `srs`, which must outlive it.  tb_verify_batch_vk takes the arguments of tb_verify_batch, has its limits, and gives the
  * same verdicts; every point of the batch is decoded on the device before the transcripts are replayed. */
-typedef struct tb_vk tb_vk;
 tb_status tb_vk_load(tb_ctx* ctx, const tb_srs* srs, const tb_cs_desc* cs, const uint8_t* fixed_commitments, const uint8_t* sigma_commitments,
                      tb_vk** out);
 void tb_vk_free(tb_vk* vk);
@@ -213,7 +229,6 @@ tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk, uint32_t n_proofs, co
  * batch as it was.  An add that fails part way (TB_ERR_CUDA) leaves the batch good only for free; finalize then refuses it.
  * Device state: n + 1 field elements and one point, on the SRS's device.  Any context on that device may use the batch, one
  * thread at a time. */
-typedef struct tb_batch_verifier tb_batch_verifier;
 tb_status tb_batch_verifier_create(tb_ctx* ctx, const tb_srs* srs, const uint8_t seed[32], tb_batch_verifier** out);
 tb_status tb_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv, const tb_vk* vk, uint32_t n_proofs,
                                 const uint8_t* instance, const uint32_t* instance_len,

@@ -190,6 +190,13 @@ class VerifyingKey {
   const Params& params() const { return *params_; }
   size_t proof_len() const { return tb_vk_proof_len(vk_.get()); }
   uint32_t num_instance() const { return num_instance_; }
+  // Proof::verify for n proofs already in device memory of the context's device (tb_dev_verify_batch_vk): proof i at
+  // d_proofs + i * proof_stride, instance values as canonical bytes, d_ok[i] written in stream order.  Returns without waiting.
+  void verify_batch_device(uint32_t n, const void* d_instance, const std::vector<uint32_t>& instance_len, const void* d_proofs, size_t proof_stride,
+                           void* d_ok) const {
+    params_->context().check(tb_dev_verify_batch_vk(params_->context().get(), vk_.get(), n, d_instance, instance_len.empty() ? nullptr : instance_len.data(),
+                                                    d_proofs, proof_stride, proof_len(), d_ok));
+  }
 
  private:
   struct Del { void operator()(tb_vk* v) const { tb_vk_free(v); } };
@@ -366,6 +373,13 @@ class BatchVerifier {
     Proof::verify_with(*params_, proofs, instances, vk.num_instance(), [&](uint32_t n, const uint8_t* inst, const uint32_t* lens, const uint8_t* buf, size_t plen, uint8_t*) {
       return tb_batch_verifier_add(params_->context().get(), bv_.get(), vk.get(), n, inst, lens, buf, plen, plen);
     });
+  }
+  // n proofs already in device memory (tb_dev_batch_verifier_add, layouts as VerifyingKey::verify_batch_device); returns
+  // without waiting
+  void add_proofs_device(const VerifyingKey& vk, uint32_t n, const void* d_instance, const std::vector<uint32_t>& instance_len, const void* d_proofs,
+                         size_t proof_stride) {
+    params_->context().check(tb_dev_batch_verifier_add(params_->context().get(), bv_.get(), vk.get(), n, d_instance,
+                                                       instance_len.empty() ? nullptr : instance_len.data(), d_proofs, proof_stride, vk.proof_len()));
   }
   bool finalize() {
     uint8_t ok = 0;

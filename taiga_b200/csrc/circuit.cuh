@@ -121,8 +121,8 @@ struct WsAlloc {
 // sum(instance_len); refuses an instance column longer than the usable rows (InstanceTooLarge)
 size_t instance_total(const Shape& C, const uint32_t* instance_len);
 // The instance columns of B proofs on the device in Montgomery form (Lagrange basis), [B][ni][n] zero past instance_len;
-// `instance` holds each proof's sum(instance_len) values column after column; refuses what instance_total refuses.  Shared by
-// the prover, the check and the verifier.
+// `instance` (a host or device pointer) holds each proof's sum(instance_len) values column after column; refuses what
+// instance_total refuses.  Shared by the prover, the check and the verifier.
 void upload_instance(Ctx* ctx, const Shape& C, int B, const uint8_t* instance, const uint32_t* instance_len, Fp* dst);
 // The witness of B proofs on the device in Montgomery form (Lagrange basis), shared by the prover and the check: the
 // instance columns as upload_instance leaves them, advice [B][na][n] (host or device pointer) whose rows >= usable are

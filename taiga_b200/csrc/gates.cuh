@@ -330,17 +330,30 @@ template <class M> TB_HD void gate_interp(M& m, int nregs, int ninstr) {
   }
 }
 
-// The host machine (the verifier at x, the CPU tests): at(kind, column, rotation) is a column query's value, ypows[i] = y^i
+// The machine at one point (the verifier at x on the host or the device, the CPU tests): at(kind, column, rotation) is a
+// column query's value, ypows[i] = y^i.  run(code, ninstr, nregs) needs regs to hold nregs + 2 values.
 template <class At> struct PointMachine {
   At at; const Fp* consts; const Fp* ypows; Fp th; Fp* lk_a; Fp* lk_s;
-  const GateProgram* p = nullptr; std::vector<Fp> regs;
-  QInstr instr(int pc) const { return pc < (int)p->code.size() ? p->code[pc] : QInstr{}; }   // gate_interp reads instruction 0 of an empty program
-  int slot(int r) const { return r; }
-  Fp get(int i) const { return regs[i]; } void set(int i, const Fp& v) { regs[i] = v; }
-  Fp leaf(int kind, uint32_t v) const { return kind == K_CONST ? consts[v] : at(kind, (int)(v >> 8), (int)(v & 255u) - 128); }
-  const Fp& ypow(uint32_t gap) const { return ypows[gap]; } const Fp& theta() const { return th; }
-  void lk_store(uint32_t l, const Fp& a, const Fp& s) { lk_a[l] = a; lk_s[l] = s; }
-  Fp run(const GateProgram& prog) { p = &prog; regs.assign(prog.nregs + 2, Fp::zero()); gate_interp(*this, prog.nregs, (int)prog.code.size()); return regs[prog.nregs]; }
+  Fp* regs = nullptr; const QInstr* code = nullptr; int ncode = 0;
+  TB_HD QInstr instr(int pc) const { return pc < ncode ? code[pc] : QInstr{}; }   // gate_interp reads instruction 0 of an empty program
+  TB_HD int slot(int r) const { return r; }
+  TB_HD Fp get(int i) const { return regs[i]; } TB_HD void set(int i, const Fp& v) { regs[i] = v; }
+  TB_HD Fp leaf(int kind, uint32_t v) const { return kind == K_CONST ? consts[v] : at(kind, (int)(v >> 8), (int)(v & 255u) - 128); }
+  TB_HD const Fp& ypow(uint32_t gap) const { return ypows[gap]; } TB_HD const Fp& theta() const { return th; }
+  TB_HD void lk_store(uint32_t l, const Fp& a, const Fp& s) { lk_a[l] = a; lk_s[l] = s; }
+  TB_HD Fp run(const QInstr* c, int ninstr, int nregs) {
+    code = c; ncode = ninstr;
+    for (int i = 0; i < nregs + 2; ++i) regs[i] = Fp::zero();
+    gate_interp(*this, nregs, ninstr);
+    return regs[nregs];
+  }
+  // host: a compiled program, with registers of its own
+  Fp run(const GateProgram& prog) {
+    std::vector<Fp> r(prog.nregs + 2);
+    Fp* keep = regs; regs = r.data();
+    Fp v = run(prog.code.data(), (int)prog.code.size(), prog.nregs);
+    regs = keep; return v;
+  }
 };
 
 }  // namespace tb

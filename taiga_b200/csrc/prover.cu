@@ -159,7 +159,7 @@ void upload_instance(Ctx* ctx, const Shape& C, int B, const uint8_t* instance, c
   for (int c = 0; c < ni; ++c) {
     if (instance_len[c])
       TB_CUDA(cudaMemcpy2DAsync(dst + (size_t)c * n, (size_t)ni * n * 32, instance + 32 * off, inst_total * 32, (size_t)instance_len[c] * 32, B,
-                                cudaMemcpyHostToDevice, ctx->stream));
+                                cudaMemcpyDefault, ctx->stream));   // host or device pointer
     off += instance_len[c];
   }
   fe_to_mont<Fp>(ctx, dst, (size_t)B * ni * n);

@@ -62,6 +62,10 @@ void powers(Ctx* c, Fp* out, long long out_stride, const Fp* x, long long x_stri
 enum ScalarOp { S_MUL = 0, S_ADD, S_SUB, S_INV, S_COPY, S_POW2K /* dst = a^(2^imm) */, S_CONST /* dst = consts[imm] */, S_NEG, S_FMA /* dst = dst*a + b */, S_POWI /* dst = a^imm */ };
 struct ScalarInstr { uint16_t op, dst, a, b; uint32_t imm; };
 void scalar_program(Ctx* c, Fp* vars, long long stride, const ScalarInstr* d_prog, int ninstr, const Fp* d_consts, int B);
+#ifdef __CUDACC__
+// v[i] = val for i < count (prover.cu)
+__global__ void fill_const_kernel(Fp* v, size_t count, Fp val);
+#endif
 
 // ---------------------------------------------------------------- verifier.cu
 // The g-terms of K proofs, added up per group of `group` consecutive proofs: G[g][t] += sum_{p in g} (ab[2p] * s_{p,t} + [t = 0]

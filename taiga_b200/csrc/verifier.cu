@@ -1,5 +1,6 @@
-// Batched verifier (SURVEY.md §8f-3): the transcript is replayed on the host, the two multi-scalar multiplications of
-// the final IPA check run on the device for the whole batch.
+// Batched verifier (SURVEY.md §8f-3): the transcript of every proof is replayed by one function (replay.cuh), on the host for
+// proofs in host memory and on the device for proofs in device memory; the two multi-scalar multiplications of the final IPA
+// check run on the device for the whole batch.
 //
 // Replaces halo2_proofs `plonk::verify_proof` with `SingleVerifier` as called by `Proof::verify`
 // (taiga_halo2/src/proof.rs:45-54; serial loop over proofs in ShieldedPartialTxBundle::execute, transaction.rs:246-257).
@@ -11,8 +12,10 @@
 #define TB_NOINLINE_MUL 1
 #include <algorithm>
 #include <cstdlib>
+#include <initializer_list>
 #include "capi_internal.cuh"
 #include "circuit.cuh"
+#include "replay.cuh"
 #include "transcript.cuh"
 
 namespace tb {
@@ -36,56 +39,148 @@ static void decompress(Ctx* ctx, const uint8_t* d_in, size_t stride, const uint3
   launch(ctx, decompress_kernel, (unsigned)((count + 127) / 128), 128, 0, d_in, stride, d_off, npts, count, d_out, d_ok);
 }
 
-// the transcript replayed over the bytes of one proof; `bad` once a read failed or the identity was absorbed.  The points
-// were decoded before the replay (pts / pts_ok: this proof's points in transcript order, at the offsets `offsets`).
-struct VTranscript : Transcript {
-  const uint8_t* rd; size_t len, pos = 0; bool bad = false;
-  const Aff<Fq>* pts; const uint8_t* pts_ok; const std::vector<uint32_t>& offsets; size_t ipt = 0;
-  VTranscript(const uint8_t* p, size_t n, const Fp& vk_repr, const Aff<Fq>* pts, const uint8_t* pts_ok, const std::vector<uint32_t>& offsets)
-      : rd(p), len(n), pts(pts), pts_ok(pts_ok), offsets(offsets) { start(vk_repr); }
-  void common_point(const Aff<Fq>& p) { if (!absorb_point(p.from_mont())) bad = true; }
-  bool read_point(Aff<Fq>& p) {
-    if (pos + 32 > len || ipt >= offsets.size()) { bad = true; return false; }
-    if (offsets[ipt] != pos) throw std::logic_error("internal error: proof point offsets");
-    if (!pts_ok[ipt]) { bad = true; return false; }
-    p = pts[ipt++]; pos += 32;
-    if (!absorb_point(p.from_mont())) bad = true;
-    return !bad;
-  }
-  bool read_scalar(Fp& s) {
-    if (pos + 32 > len || !canonical<Fp>(rd + pos, s)) { bad = true; return false; }
-    pos += 32; absorb_scalar(s.from_mont()); return true;
-  }
-};
-
-__global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_t* ok, int K) {
+// ok[p] = 1 iff a[p] + b[p] is the identity and (alive = nullptr or) alive[p] != 0
+__global__ void verify_final_kernel(const Xyzz<Fq>* a, const Xyzz<Fq>* b, uint8_t* ok, int K, const uint8_t* alive) {
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= K) return;
   Xyzz<Fq> s = a[p]; s.add(b[p]);
-  ok[p] = s.is_inf() ? 1 : 0;
+  ok[p] = (s.is_inf() && (!alive || alive[p])) ? 1 : 0;
 }
 
-// the proof's evaluations at x (C.evals order, then the expected h(x)), as argument.cuh reads them
-struct EvalView {
-  const Shape& C; const std::vector<Fp>& ev; int last_rot;
-  Fp at(const PolyId& poly, int rot) const { return ev[C.eval_index(poly, rot)]; }
-  Fp perm_col(int c) const { return at(column_poly(C.perm[c]), 0); }
-  Fp sigma(int c) const { return at({PK_SIG, c}, 0); }
-  Fp z(int s) const { return at({PK_PZ, s}, 0); }
-  Fp z_next(int s) const { return at({PK_PZ, s}, 1); }
-  Fp z_last(int s) const { return at({PK_PZ, s}, last_rot); }
-};
-
 // commit_lagrange(column, Blind::default()) of `count` columns of n values at `vals` ([count][n], Montgomery): the points,
-// Montgomery, on the host
+// Montgomery, on the device at `out`
+static void commit_columns_dev(Ctx* ctx, const Srs& srs, const Fp* vals, int count, Aff<Fq>* out) {
+  if (!count) return;
+  DevBuf<Fp> ones(ctx, count);
+  launch(ctx, fill_const_kernel, (unsigned)((count + 127) / 128), 128, 0, ones.get(), (size_t)count, Fp::one());
+  srs.commit(ctx, true, vals, (long long)srs.n, count, ones.get(), out);
+}
+// the same, on the host
 static std::vector<Aff<Fq>> commit_columns(Ctx* ctx, const Srs& srs, const Fp* vals, int count) {
   std::vector<Aff<Fq>> out(count, Aff<Fq>::inf());
   if (!count) return out;
-  DevBuf<Fp> ones(ctx, count); DevBuf<Aff<Fq>> pts(ctx, count);
-  std::vector<Fp> h(count, Fp::one()); ones.upload(h.data(), count);
-  srs.commit(ctx, true, vals, (long long)srs.n, count, ones.get(), pts.get());
+  DevBuf<Aff<Fq>> pts(ctx, count);
+  commit_columns_dev(ctx, srs, vals, count, pts.get());
   pts.download(out.data(), count); ctx->sync();
   return out;
+}
+
+// The ReplayShape of a shape with its tables packed in `blob`: until bind(base) its pointers are offsets into the blob, so
+// one copy of the blob (host or device) serves the replay.  Building it checks, once per call, what the replay relies on:
+// every evaluation it reads exists, the points lie at the offsets it reads them from, and it pushes exactly M terms.
+struct ReplayPlan {
+  ReplayShape v;
+  std::vector<uint8_t> blob;
+  template <class T> const T* put(const T* p, size_t n) {
+    const size_t off = (blob.size() + 15) & ~size_t(15);
+    blob.resize(off + std::max<size_t>(1, n) * sizeof(T));
+    if (n) memcpy(blob.data() + off, p, n * sizeof(T));
+    return reinterpret_cast<const T*>(off);
+  }
+  template <class T> const T* put(const std::vector<T>& x) { return put(x.data(), x.size()); }
+  template <class T> static const T* at(const uint8_t* base, const T* off) { return reinterpret_cast<const T*>(base + reinterpret_cast<uintptr_t>(off)); }
+  ReplayShape bind(const uint8_t* base) const {
+    ReplayShape s = v;
+    s.rots = at(base, s.rots); s.evpos = at(base, s.evpos); s.uniq = at(base, s.uniq); s.ps_off = at(base, s.ps_off); s.ps_rot = at(base, s.ps_rot);
+    s.perm_kind = at(base, s.perm_kind); s.perm_idx = at(base, s.perm_idx); s.progs = at(base, s.progs); s.code = at(base, s.code); s.consts = at(base, s.consts);
+    return s;
+  }
+};
+static_assert((int)PK_INST == RP_INST && (int)PK_ADV == RP_ADV && (int)PK_PZ == RP_PZ && (int)PK_LZ == RP_LZ && (int)PK_LPIN == RP_LPIN && (int)PK_LPTAB == RP_LPTAB && (int)PK_FIXED == RP_FIXED &&
+              (int)PK_SIG == RP_SIG && (int)PK_H == RP_H && (int)PK_RANDOM == RP_RANDOM, "replay.cuh numbers polynomials as circuit.cuh does");
+
+static ReplayPlan replay_plan(const Shape& C) {
+  auto internal = [](bool cond, const char* what) { if (!cond) throw std::logic_error(std::string("internal error: ") + what); };
+  ReplayPlan R; ReplayShape& v = R.v;
+  v.k = (int)C.k; v.na = (int)C.na; v.ni = (int)C.ni; v.L = (int)C.L; v.nsets = (int)C.nsets; v.P = (int)C.P; v.bf = (int)C.bf; v.pieces = (int)C.pieces;
+  v.chunk = (int)C.chunk; v.nevals = (int)C.evals.size(); v.nuniq = (int)C.uniq.size(); v.nps = (int)C.point_sets.size(); v.npts = (int)C.point_offsets.size();
+  v.proof_len = C.proof_len;
+  v.vk_repr = C.vk_repr; v.omega = C.omega; v.omega_inv = C.omega.inv(); v.n_inv = Fp::from_u32((uint32_t)C.n).inv(); v.delta = C.delta;
+  for (int s = 0; s < PERM_MAX_SETS; ++s) v.delta_c0[s] = C.delta_c0[s];
+  // (poly, rotation) -> evaluation, dense
+  const int counts[RP_KINDS] = {v.ni, v.na, v.nsets, v.L, v.L, v.L, (int)C.nf, v.P, 1, 1};
+  int npoly = 0;
+  for (int kd = 0; kd < RP_KINDS; ++kd) { v.poly_base[kd] = npoly; npoly += counts[kd]; }
+  const std::vector<int>& rots = C.rots; v.nrots = (int)rots.size();
+  auto rot_index = [&](int rot) { return (int)(std::find(rots.begin(), rots.end(), rot) - rots.begin()); };
+  std::vector<int> evpos((size_t)npoly * v.nrots, -1);
+  for (const auto& kv : C.eval_pos) {
+    const int r = rot_index(kv.first.second);
+    internal(r < v.nrots && kv.first.first.idx < counts[kv.first.first.kind], "an evaluation outside the replay's table");
+    evpos[(size_t)(v.poly_base[kv.first.first.kind] + kv.first.first.idx) * v.nrots + r] = kv.second;
+  }
+  auto need = [&](int kind, int idx, int rot) {
+    const int r = rot_index(rot);
+    internal(idx >= 0 && idx < counts[kind] && r < v.nrots && evpos[(size_t)(v.poly_base[kind] + idx) * v.nrots + r] >= 0, "a query without an evaluation");
+  };
+  // the multiopen's commitments and point sets
+  const int na = v.na, L = v.L, nsets = v.nsets, commits = na + 3 * L + nsets + 1 + v.pieces;
+  std::vector<RpUniq> uniq; int nh = 0;
+  for (int c = 0; c < v.nuniq; ++c) {
+    const PolyId& id = C.uniq[c]; const int s = C.uniq_set[c];
+    int src = -1;
+    switch (id.kind) {
+      case PK_ADV: src = id.idx; break;
+      case PK_LPIN: src = na + 2 * id.idx; break;
+      case PK_LPTAB: src = na + 2 * id.idx + 1; break;
+      case PK_PZ: src = na + 2 * L + id.idx; break;
+      case PK_LZ: src = na + 2 * L + nsets + id.idx; break;
+      case PK_RANDOM: src = na + 2 * L + nsets + L; break;
+      case PK_H: src = na + 2 * L + nsets + L + 1; ++nh; break;
+      default: break;
+    }
+    uniq.push_back({id.kind, id.idx, s, src});
+    for (int rot : C.point_sets[s]) need(id.kind, id.idx, rot);
+  }
+  std::vector<int> ps_off(1, 0), ps_rot; int max_set = 1;
+  for (const auto& ps : C.point_sets) { ps_rot.insert(ps_rot.end(), ps.begin(), ps.end()); ps_off.push_back((int)ps_rot.size()); max_set = std::max(max_set, (int)ps.size()); }
+  // the arguments' reads
+  std::vector<int> perm_kind, perm_idx;
+  for (int c = 0; c < v.P; ++c) {
+    const PolyId id = column_poly(C.perm[c]);
+    perm_kind.push_back(id.kind); perm_idx.push_back(id.idx);
+    need(id.kind, id.idx, 0); need(PK_SIG, c, 0);
+  }
+  for (int s = 0; s < nsets; ++s) { need(PK_PZ, s, 0); need(PK_PZ, s, 1); if (s + 1 < nsets) need(PK_PZ, s, -(v.bf + 1)); }
+  for (int l = 0; l < L; ++l) { need(PK_LZ, l, 0); need(PK_LZ, l, 1); need(PK_LPIN, l, 0); need(PK_LPIN, l, -1); need(PK_LPTAB, l, 0); }
+  need(PK_H, 0, 0);
+  // the gate programs, then the lookup program, with every column query they read
+  std::vector<RpProgram> progs; std::vector<QInstr> code; int max_regs = 0;
+  auto add = [&](const GateProgram& g) {
+    progs.push_back({(int)code.size(), (int)g.code.size(), g.nregs, g.last});
+    max_regs = std::max(max_regs, g.nregs);
+    for (const QInstr& in : g.code) {
+      const int kinds[2] = {(int)((in.w0 >> 16) & 0xff), (int)(in.w0 >> 24)}; const uint32_t vals[2] = {in.a, in.b};
+      for (int o = 0; o < 2; ++o)
+        if (kinds[o] == K_ADV || kinds[o] == K_FIX || kinds[o] == K_INST)
+          need(kinds[o] == K_ADV ? PK_ADV : kinds[o] == K_FIX ? PK_FIXED : PK_INST, (int)(vals[o] >> 8), (int)(vals[o] & 255u) - 128);
+      code.push_back(in);
+    }
+  };
+  for (const auto* parts : {&C.plan.gate_parts[0], &C.plan.gate_parts_lo[0]})
+    for (const GateProgram& g : *parts) add(g);
+  v.ngates = (int)progs.size();
+  add(C.plan.lookups);
+  v.J = (int)C.plan.num_constraints; v.nypow = v.J + (int)C.plan.t_pl + 2;
+  // the proof's layout: the commitments, the evaluations, q', the multiopen evaluations u, S, then k (L, R) pairs and (c, f)
+  { std::vector<uint32_t> off; uint32_t pos = 0;
+    for (int i = 0; i < commits; ++i, pos += 32) off.push_back(pos);
+    pos += 32 * v.nevals; off.push_back(pos); pos += 32 + 32 * v.nps; off.push_back(pos); pos += 32;
+    for (int j = 0; j < 2 * v.k; ++j, pos += 32) off.push_back(pos);
+    pos += 64;
+    internal(off == C.point_offsets && pos == C.proof_len, "proof point offsets"); }
+  // every committed polynomial (h in its pieces), q', S, the L_j and R_j, W and U
+  v.M = v.nuniq - 1 + v.pieces + 2 + 2 * v.k + 2;
+  internal(nh == 1, "verifier term count");
+  v.rots = R.put(rots); v.evpos = R.put(evpos); v.uniq = R.put(uniq); v.ps_off = R.put(ps_off); v.ps_rot = R.put(ps_rot);
+  v.perm_kind = R.put(perm_kind); v.perm_idx = R.put(perm_idx); v.progs = R.put(progs); v.code = R.put(code); v.consts = R.put(C.consts_host);
+  // scratch per proof
+  int s = 0;
+  auto carve = [&](int count) { const int at = s; s += std::max(1, count); return at; };
+  v.s_ev = carve(v.nevals + 1); v.s_regs = carve(max_regs + 2); v.s_ypow = carve(v.nypow); v.s_lka = carve(L); v.s_lkt = carve(L);
+  v.s_qev = carve(ps_off.back()); v.s_coef = carve(v.nuniq); v.s_cur = carve(v.nps); v.s_u = carve(v.nps); v.s_x4 = carve(v.nps + 1); v.s_ptsx = carve(max_set);
+  v.scratch = s;
+  return R;
 }
 
 // What the transcript replay of K proofs leaves for their final IPA checks.  Proof p's M variable-base terms are pts / sc at
@@ -97,15 +192,17 @@ struct Replay {
   std::vector<Aff<Fq>> pts; std::vector<Fp> sc, us, ab; std::vector<char> alive;
 };
 
-// Replays the transcripts of K proofs of proof_len == C.proof_len bytes of the circuit of shape C, whose fixed / sigma
-// commitments are `vk_fixed` / `vk_sigma` (Montgomery).  Every point is decoded and every instance column committed on the
-// device first.
+// Replays, on the host, the transcripts of K proofs (host memory) of proof_len == C.proof_len bytes of the circuit of shape C,
+// whose fixed / sigma commitments are `vk_fixed` / `vk_sigma` (Montgomery).  Every point is decoded and every instance column
+// committed on the device first.
 static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
                          const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, Replay& rep) {
-  const size_t n = C.n; const int kk = (int)C.k, na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf, pieces = C.pieces;
+  const ReplayPlan plan = replay_plan(C);
+  const ReplayShape S = plan.bind(plan.blob.data());
+  const int kk = (int)C.k, ni = C.ni;
   const size_t inst_total = instance_total(C, instance_len);
   // ---- every point of the batch, decoded on the device: [K][npts]
-  const int npts = (int)C.point_offsets.size();
+  const int npts = S.npts;
   std::vector<Aff<Fq>> dec((size_t)K * npts);
   std::vector<uint8_t> dec_ok((size_t)K * npts);
   { DevBuf<uint8_t> d_proofs(ctx, (size_t)K * proof_len), d_ok(ctx, dec_ok.size()); DevBuf<uint32_t> d_off(ctx, npts); DevBuf<Aff<Fq>> d_pts(ctx, dec.size());
@@ -116,127 +213,80 @@ static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
   // ---- instance commitments for the whole batch: [K][ni]
   std::vector<Aff<Fq>> inst_comm;
   if (ni) {
-    DevBuf<Fp> iv(ctx, (size_t)K * ni * n);
+    DevBuf<Fp> iv(ctx, (size_t)K * ni * C.n);
     upload_instance(ctx, C, K, instance, instance_len, iv.get());
     inst_comm = commit_columns(ctx, srs, iv.get(), K * ni);
   }
-  // ---- per proof: replay the transcript, accumulate (scalar, point) pairs
-  const int nps = (int)C.point_sets.size();
-  // variable-base terms per proof: every committed polynomial (h in its pieces), q', S, the L_j and R_j, W and U
-  rep.M = (int)C.uniq.size() - 1 + pieces + 2 + 2 * kk + 2;
+  // ---- per proof: the shared replay
+  rep.M = S.M;
   rep.pts.assign((size_t)K * rep.M, Aff<Fq>::inf());
   rep.sc.assign((size_t)K * rep.M, Fp::zero()); rep.us.assign((size_t)K * kk, Fp::zero()); rep.ab.assign((size_t)K * 2, Fp::zero());
   rep.alive.assign(K, 0);
-  const Fp one = Fp::one();
-  const int last_rot = -(bf + 1);
-  Fp omega = C.omega, omega_inv = C.omega.inv(), n_inv = Fp::from_u32((uint32_t)n).inv();
-  auto rot_pow = [&](int rot) { Fp r = one; const Fp& w = rot >= 0 ? omega : omega_inv; for (int i = 0; i < std::abs(rot); ++i) r = r * w; return r; };
+  std::vector<Fp> scratch(S.scratch);
   for (int p = 0; p < K; ++p) {
-    VTranscript tr(proofs + (size_t)p * proof_stride, proof_len, C.vk_repr, dec.data() + (size_t)p * npts, dec_ok.data() + (size_t)p * npts, C.point_offsets);
-    bool ok = true;
-    const uint8_t* ib = instance + 32 * inst_total * p;
-    for (size_t i = 0; i < inst_total && ok; ++i) { Fp t; ok = canonical<Fp>(ib + 32 * i, t); }
-    if (!ok) continue;
-    // commitment table for this proof: id -> point
-    std::map<PolyId, Aff<Fq>> comm;
-    for (int c = 0; c < ni; ++c) { comm[{PK_INST, c}] = inst_comm[(size_t)p * ni + c]; tr.common_point(inst_comm[(size_t)p * ni + c]); }
-    auto rp = [&](PolyId id) { Aff<Fq> pt; if (!tr.read_point(pt)) return false; comm[id] = pt; return true; };
-    for (int c = 0; c < na && ok; ++c) ok = rp({PK_ADV, c});
-    Fp theta = tr.squeeze();
-    for (int l = 0; l < L && ok; ++l) ok = rp({PK_LPIN, l}) && rp({PK_LPTAB, l});
-    Fp beta = tr.squeeze(), gamma = tr.squeeze();
-    for (int s = 0; s < nsets && ok; ++s) ok = rp({PK_PZ, s});
-    for (int l = 0; l < L && ok; ++l) ok = rp({PK_LZ, l});
-    ok = ok && rp({PK_RANDOM, 0});
-    Fp y = tr.squeeze();
-    std::vector<Aff<Fq>> hpts(pieces);
-    for (int i = 0; i < pieces && ok; ++i) ok = tr.read_point(hpts[i]);
-    Fp x = tr.squeeze();
-    if (!ok) continue;
-    // evaluations, in the prover's order (C.evals); the last entry is set to the expected h(x) below
-    std::vector<Fp> ev(C.evals.size() + 1, Fp::zero());
-    for (size_t i = 0; i < C.evals.size() && ok; ++i) ok = tr.read_scalar(ev[i]);
-    if (!ok) continue;
-    const EvalView view{C, ev, last_rot};
-    // expected h(x)
-    Fp xn = x; for (int i = 0; i < kk; ++i) xn = xn.sqr();
-    auto l_at = [&](int rot) { Fp wi = rot_pow(rot); return (xn - one) * n_inv * wi * (x - wi).inv(); };
-    Fp l_last = l_at(last_rot), l_blind = Fp::zero(), l_0 = l_at(0);
-    for (int r = -bf; r <= -1; ++r) l_blind = l_blind + l_at(r);
-    // the circuit's programs at x: the gates as the quotient combines its parts (sum_p y^(J - 1 - last_p) S_p), and the lookups
-    const int J = (int)C.plan.num_constraints;
-    std::vector<Fp> ypow(J + C.plan.t_pl + 2, one), lk_a(L), lk_t(L);
-    for (size_t i = 1; i < ypow.size(); ++i) ypow[i] = ypow[i - 1] * y;
-    auto at_x = [&](int kind, int col, int rot) { return view.at({kind == K_ADV ? PK_ADV : kind == K_FIX ? PK_FIXED : PK_INST, col}, rot); };
-    PointMachine<decltype(at_x)> m{at_x, C.consts_host.data(), ypow.data(), theta, lk_a.data(), lk_t.data()};
-    Fp acc = Fp::zero();
-    for (const auto* parts : {&C.plan.gate_parts[0], &C.plan.gate_parts_lo[0]})
-      for (const GateProgram& g : *parts) acc = acc + ypow[J - 1 - g.last] * m.run(g);
-    m.run(C.plan.lookups);
-    const ArgPoint at = {y, beta, gamma, l_0, l_last, one - (l_last + l_blind)};
-    acc = perm_fold(acc, view, at, nsets, (int)C.chunk, P, C.delta, C.delta_c0, x);
-    for (int l = 0; l < L; ++l)
-      acc = lookup_fold(acc, at, view.at({PK_LZ, l}, 0), view.at({PK_LZ, l}, 1), view.at({PK_LPIN, l}, 0), view.at({PK_LPIN, l}, -1), view.at({PK_LPTAB, l}, 0),
-                        lk_a[l], lk_t[l]);
-    ev[C.eval_index({PK_H, 0}, 0)] = acc * (xn - one).inv();
-    // ---- multiopen
-    Fp x1 = tr.squeeze(), x2 = tr.squeeze();
-    std::vector<std::vector<Fp>> q_evals(nps);
-    for (int s = 0; s < nps; ++s) q_evals[s].assign(C.point_sets[s].size(), Fp::zero());
-    std::map<PolyId, Fp> coef_in_set;   // coefficient of each commitment inside its q_commitment (power of x1)
-    { std::vector<Fp> cur(nps, one); std::vector<char> started(nps, 0);
-      // q_comm[s] = (...(C_first * x1 + C_2) * x1 + ...) : walk backwards so each commitment gets x1^(#later ones in its set)
-      for (int c = (int)C.uniq.size() - 1; c >= 0; --c) { int s = C.uniq_set[c]; coef_in_set[C.uniq[c]] = cur[s]; cur[s] = cur[s] * x1; }
-      for (size_t c = 0; c < C.uniq.size(); ++c) {
-        int s = C.uniq_set[c];
-        for (size_t pi = 0; pi < C.point_sets[s].size(); ++pi) q_evals[s][pi] = q_evals[s][pi] * x1 + view.at(C.uniq[c], C.point_sets[s][pi]);
-      } }
-    Aff<Fq> q_prime; ok = ok && tr.read_point(q_prime);
-    Fp x3 = tr.squeeze();
-    std::vector<Fp> u(nps); for (auto& e : u) ok = ok && tr.read_scalar(e);
-    if (!ok) continue;
-    Fp msm_eval = Fp::zero();
-    for (int s = 0; s < nps; ++s) {
-      size_t m = C.point_sets[s].size();
-      std::vector<Fp> ptsx(m); for (size_t i = 0; i < m; ++i) ptsx[i] = x * rot_pow(C.point_sets[s][i]);
-      Fp r_eval = Fp::zero();
-      for (size_t i = 0; i < m; ++i) { Fp num = one, den = one; for (size_t j = 0; j < m; ++j) if (j != i) { num = num * (x3 - ptsx[j]); den = den * (ptsx[i] - ptsx[j]); } r_eval = r_eval + q_evals[s][i] * num * den.inv(); }
-      Fp e = u[s] - r_eval;
-      for (size_t i = 0; i < m; ++i) e = e * (x3 - ptsx[i]).inv();
-      msm_eval = msm_eval * x2 + e;
-    }
-    Fp x4 = tr.squeeze();
-    std::vector<Fp> x4pow(nps + 1, one); for (int i = 1; i <= nps; ++i) x4pow[i] = x4pow[i - 1] * x4;
-    Fp v = msm_eval * x4pow[nps];
-    for (int s = 0; s < nps; ++s) v = v + u[s] * x4pow[nps - 1 - s];
-    // ---- IPA part of the transcript
-    Aff<Fq> s_comm; ok = ok && tr.read_point(s_comm);
-    Fp xi = tr.squeeze(), z = tr.squeeze();
-    std::vector<Aff<Fq>> Ls(kk), Rs(kk); std::vector<Fp> uj(kk);
-    for (int j = 0; j < kk && ok; ++j) { ok = tr.read_point(Ls[j]) && tr.read_point(Rs[j]); uj[j] = tr.squeeze(); }
-    Fp cc, ff; ok = ok && tr.read_scalar(cc) && tr.read_scalar(ff);
-    if (!ok || tr.bad || tr.pos != proof_len) continue;
-    Fp b = one; { Fp cur = x3; for (int j = kk - 1; j >= 0; --j) { b = b * (one + uj[j] * cur); cur = cur * cur; } }
-    // ---- variable-base terms
-    Aff<Fq>* pp = rep.pts.data() + (size_t)p * rep.M; Fp* ss = rep.sc.data() + (size_t)p * rep.M; int w = 0;
-    auto push = [&](const Aff<Fq>& pt, const Fp& sc) { pp[w] = pt; ss[w] = sc; ++w; };
-    for (size_t c = 0; c < C.uniq.size(); ++c) {
-      const PolyId& id = C.uniq[c]; Fp coef = coef_in_set[id] * x4pow[nps - 1 - C.uniq_set[c]];
-      if (id.kind == PK_H) { Fp cur = coef; for (int i = 0; i < pieces; ++i) { push(hpts[i], cur); cur = cur * xn; } }
-      else if (id.kind == PK_FIXED) push(vk_fixed[id.idx], coef);
-      else if (id.kind == PK_SIG) push(vk_sigma[id.idx], coef);
-      else push(comm[id], coef);
-    }
-    push(q_prime, x4pow[nps]);
-    push(s_comm, xi);
-    for (int j = 0; j < kk; ++j) { push(Ls[j], uj[j].inv()); push(Rs[j], uj[j]); }
-    push(srs.w_host, ff.neg());
-    push(srs.u_host, (cc * b * z).neg());
-    if (w != rep.M) throw std::logic_error("internal error: verifier term count");
-    for (int j = 0; j < kk; ++j) rep.us[(size_t)p * kk + j] = uj[j];
-    rep.ab[2 * p] = cc.neg(); rep.ab[2 * p + 1] = v.neg();
-    rep.alive[p] = 1;
+    const ReplayIn in = {proofs + (size_t)p * proof_stride, proof_len, dec.data() + (size_t)p * npts, dec_ok.data() + (size_t)p * npts,
+                         instance + 32 * inst_total * p, inst_total, ni ? inst_comm.data() + (size_t)p * ni : nullptr, vk_fixed.data(), vk_sigma.data(),
+                         srs.w_host, srs.u_host};
+    const ReplayOut out = {rep.pts.data() + (size_t)p * rep.M, rep.sc.data() + (size_t)p * rep.M, rep.us.data() + (size_t)p * kk, rep.ab.data() + 2 * p};
+    rep.alive[p] = replay_proof(S, in, scratch.data(), out) ? 1 : 0;
   }
+}
+
+// One thread per proof: the shared replay over device memory.  A proof rejected during its replay gets alive[p] = 0 and, when
+// batch_alive is given, sets *batch_alive = 0.
+constexpr int RP_THREADS = 32;
+__global__ void __launch_bounds__(RP_THREADS) replay_kernel(const ReplayShape S, int K, const uint8_t* __restrict__ proofs, size_t stride, size_t len,
+                                                            const uint8_t* __restrict__ inst, size_t inst_total, const Aff<Fq>* __restrict__ dec,
+                                                            const uint8_t* __restrict__ dec_ok, const Aff<Fq>* __restrict__ inst_comm,
+                                                            const Aff<Fq>* __restrict__ fixed, const Aff<Fq>* __restrict__ sigma, const Aff<Fq>* __restrict__ wu,
+                                                            Fp* __restrict__ scratch, Aff<Fq>* __restrict__ pts, Fp* __restrict__ sc, Fp* __restrict__ us,
+                                                            Fp* __restrict__ ab, uint8_t* __restrict__ alive, uint8_t* batch_alive) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= K) return;
+  const ReplayIn in = {proofs + (size_t)p * stride, len, dec + (size_t)p * S.npts, dec_ok + (size_t)p * S.npts, inst + 32 * inst_total * p, inst_total,
+                       inst_comm + (size_t)p * S.ni, fixed, sigma, wu[0], wu[1]};
+  const ReplayOut out = {pts + (size_t)p * S.M, sc + (size_t)p * S.M, us + (size_t)p * S.k, ab + 2 * p};
+  const bool good = replay_proof(S, in, scratch + (size_t)p * S.scratch, out);
+  alive[p] = good ? 1 : 0;
+  if (!good && batch_alive) *batch_alive = 0;
+}
+
+// What the device replay of K proofs leaves, as Replay, on the device
+struct DevReplay {
+  int M = 0;
+  DevBuf<Aff<Fq>> pts; DevBuf<Fp> sc, us, ab; DevBuf<uint8_t> alive;
+};
+
+// The replay of K proofs in device memory (proof p at d_proofs + p * proof_stride, proof_len == the shape's), enqueued on the
+// context's stream: the points decoded, the instance columns committed, then replay_kernel.  Nothing is waited for.
+static void replay_batch_dev(Ctx* ctx, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len, const uint8_t* d_proofs,
+                             size_t proof_stride, size_t proof_len, DevReplay& r, uint8_t* batch_alive) {
+  const Shape& C = vk.shape; const Srs& srs = *vk.srs;
+  const int ni = C.ni;
+  const size_t inst_total = instance_total(C, instance_len);
+  // the shape's tables, the key's commitments and the point offsets: one upload
+  ReplayPlan plan = replay_plan(C);
+  const Aff<Fq>* o_fixed = plan.put(vk.fixed); const Aff<Fq>* o_sigma = plan.put(vk.sigma); const uint32_t* o_off = plan.put(C.point_offsets);
+  DevBuf<uint8_t> d_blob(ctx, plan.blob.size());
+  d_blob.upload(plan.blob.data(), plan.blob.size());
+  const ReplayShape S = plan.bind(d_blob.get());
+  const int npts = S.npts;
+  DevBuf<Aff<Fq>> dec(ctx, (size_t)K * npts); DevBuf<uint8_t> dec_ok(ctx, (size_t)K * npts);
+  decompress(ctx, d_proofs, proof_stride, ReplayPlan::at(d_blob.get(), o_off), npts, (size_t)K * npts, dec.get(), dec_ok.get());
+  DevBuf<Aff<Fq>> inst_comm(ctx, (size_t)K * ni);
+  if (ni) {
+    DevBuf<Fp> iv(ctx, (size_t)K * ni * C.n);
+    upload_instance(ctx, C, K, d_instance, instance_len, iv.get());
+    commit_columns_dev(ctx, srs, iv.get(), K * ni, inst_comm.get());
+  }
+  r.M = S.M;
+  r.pts = DevBuf<Aff<Fq>>(ctx, (size_t)K * S.M); r.sc = DevBuf<Fp>(ctx, (size_t)K * S.M); r.us = DevBuf<Fp>(ctx, (size_t)K * C.k);
+  r.ab = DevBuf<Fp>(ctx, (size_t)K * 2); r.alive = DevBuf<uint8_t>(ctx, K);
+  DevBuf<Fp> scratch(ctx, (size_t)K * S.scratch);
+  ProfScope scope(ctx, PC_TRANSCRIPT);
+  launch(ctx, replay_kernel, (unsigned)((K + RP_THREADS - 1) / RP_THREADS), RP_THREADS, 0, S, K, d_proofs, proof_stride, proof_len, d_instance, inst_total,
+         dec.get(), dec_ok.get(), inst_comm.get(), ReplayPlan::at(d_blob.get(), o_fixed), ReplayPlan::at(d_blob.get(), o_sigma), srs.wu.get(), scratch.get(),
+         r.pts.get(), r.sc.get(), r.us.get(), r.ab.get(), r.alive.get(), batch_alive);
 }
 
 // n_proofs proofs of the circuit of shape C, each checked on its own: the replay, then both MSMs of every proof's final
@@ -256,26 +306,52 @@ static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::ve
   msm_run<Fq, Fp>(ctx, d_sc.get(), r.M, d_pts.get(), r.M, r.M, K, MsmConfig(), acc_v.get());
   batch_g_scalars(ctx, d_gs.get(), d_us.get(), d_ab.get(), (int)C.k, K, 1);
   srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
-  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K);
+  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K, (const uint8_t*)nullptr);
   std::vector<uint8_t> hok(K);
   d_ok.download(hok.data(), K); ctx->sync();
   for (int p = 0; p < K; ++p) ok_out[p] = (r.alive[p] && hok[p]) ? 1 : 0;
+}
+
+// The same for proofs, instance values and verdicts in device memory, enqueued on the context's stream without waiting:
+// d_ok_out[p] = 1 iff proof p is accepted.  A proof_len other than the shape's gives 0 for every proof, nothing decoded.
+static void verify_batch_dev(Ctx* ctx, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len, const uint8_t* d_proofs,
+                             size_t proof_stride, size_t proof_len, uint8_t* d_ok_out) {
+  const Shape& C = vk.shape; const size_t n = C.n;
+  if (proof_len != C.proof_len) { TB_CUDA(cudaMemsetAsync(d_ok_out, 0, K, ctx->stream)); return; }
+  DevReplay r;
+  replay_batch_dev(ctx, vk, K, d_instance, instance_len, d_proofs, proof_stride, proof_len, r, nullptr);
+  DevBuf<Fp> d_gs(ctx, (size_t)K * n); DevBuf<Xyzz<Fq>> acc_v(ctx, K), acc_g(ctx, K);
+  d_gs.zero();
+  msm_run<Fq, Fp>(ctx, r.sc.get(), r.M, r.pts.get(), r.M, r.M, K, MsmConfig(), acc_v.get());
+  batch_g_scalars(ctx, d_gs.get(), r.us.get(), r.ab.get(), (int)C.k, K, 1);
+  vk.srs->commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
+  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok_out, K, (const uint8_t*)r.alive.get());
 }
 
 // ---------------------------------------------------------------- batch verifier (tb_batch_verifier)
 // halo2's BatchVerifier: proof j's final-check sum is weighted by rho_j = PRF(seed, j, R_BATCH_WEIGHT, 0) and the weighted sums
 // of every proof added are added up, so one test for the identity decides the whole batch.  All proofs commit over one SRS,
 // so their g-terms share `g` (n scalars); everything else of a call's proofs goes through one variable-base MSM whose result
-// is added into `acc`.  `next` is the j of the next proof; `rejected`: a proof was rejected before its final check.
+// is added into `acc`.  `next` is the j of the next proof; `rejected`: a proof was rejected before its final check on the host,
+// `alive` = 0: one was rejected during a device replay.
 struct BatchVerifier {
   const Srs* srs = nullptr; int device = 0; uint8_t seed[32];
   uint64_t next = 0;
   bool rejected = false;
   bool broken = false;      // an add failed after it began changing g / acc: only tb_batch_verifier_free is allowed
   bool finalized = false;
+  const Ctx* pending = nullptr;   // the context whose stream may still hold device adds (compared, never dereferenced)
   DevMem<Fp> g;             // [n] sum_p rho_p (-c_p s_{p,t} - [t = 0] v_p), Montgomery
   DevMem<Xyzz<Fq>> acc;     // [1] sum_p rho_p (every variable-base term of proof p, W and U included)
+  DevMem<uint8_t> alive;    // [1] 1 until a device replay rejects a proof
 };
+
+// Before `ctx` works on the batch: device adds another context enqueued must have run.  That context may be closed by now,
+// so the whole device is waited for; a batch that stays on one context never waits here.
+static void batch_claim(const Ctx* ctx, BatchVerifier& bv) {
+  if (bv.pending && bv.pending != ctx) TB_CUDA(cudaDeviceSynchronize());
+  bv.pending = nullptr;
+}
 
 // Per proof p of a call (one CTA each): its M variable-base scalars and ab[p], the coefficients of its g-term, times rho_p
 __global__ void batch_weights_kernel(const Fp* __restrict__ rho, Fp* __restrict__ sc, int M, Fp* __restrict__ ab) {
@@ -334,12 +410,26 @@ void batch_g_scalars(Ctx* ctx, Fp* G, const Fp* us, const Fp* ab, int kk, int K,
   launch(ctx, batch_g_scalars_kernel, dim3(1u << (kk - lb), (unsigned)((K - 1) / group + 1)), BG_THREADS, 0, G, us, ab, kk, K, group);
 }
 
-// The proofs of one tb_batch_verifier_add: replay, then (unless a proof was rejected) their weights, their terms through one
-// variable-base MSM into bv.acc, and their g-terms into bv.g.
+// Adds K replayed proofs (device terms pts / sc, M per proof, us, ab) of a circuit of k rows to the batch: their weights
+// rho_{j0 + p}, their terms through one variable-base MSM into bv.acc, their g-terms into bv.g.  sc and ab are scaled in place.
+static void batch_fold(Ctx* ctx, BatchVerifier& bv, uint32_t j0, int K, int M, int kk, const Aff<Fq>* pts, Fp* sc, const Fp* us, Fp* ab) {
+  DevBuf<Fp> d_rho(ctx, K); DevBuf<Xyzz<Fq>> part(ctx, 1);
+  { ProfScope scope(ctx, PC_IPA_FOLD);
+    prf_fill(ctx, bv.seed, j0, R_BATCH_WEIGHT, 0, d_rho.get(), 1, 1, 1, K);
+    ctx->work[PC_IPA_FOLD] += (double)K * (M + 2);
+    launch(ctx, batch_weights_kernel, K, 128, 0, d_rho.get(), sc, M, ab); }
+  msm_run<Fq, Fp>(ctx, sc, 0, pts, 0, K * M, 1, MsmConfig(), part.get());
+  { ProfScope scope(ctx, PC_MSM_REDUCE);
+    launch(ctx, batch_acc_kernel, 1, 1, 0, bv.acc.get(), part.get()); }
+  batch_g_scalars(ctx, bv.g.get(), us, ab, kk, K, K);
+}
+
+// The proofs of one tb_batch_verifier_add: replay on the host, then (unless a proof was rejected) batch_fold
 static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K, const uint8_t* instance, const uint32_t* instance_len,
                       const uint8_t* proofs, size_t proof_stride, size_t proof_len) {
   const Shape& C = vk.shape;
   const uint32_t j0 = (uint32_t)bv.next;
+  batch_claim(ctx, bv);
   if (!bv.rejected && proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted
   if (!bv.rejected) {
     Replay r;
@@ -347,18 +437,10 @@ static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K
     if (std::find(r.alive.begin(), r.alive.end(), 0) != r.alive.end()) bv.rejected = true;
     else {
       const size_t N = (size_t)K * r.M;
-      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_rho(ctx, K), d_ab(ctx, r.ab.size());
-      DevBuf<Xyzz<Fq>> part(ctx, 1);
+      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_ab(ctx, r.ab.size());
       d_pts.upload(r.pts.data(), N); d_sc.upload(r.sc.data(), N); d_us.upload(r.us.data(), r.us.size()); d_ab.upload(r.ab.data(), r.ab.size());
       bv.broken = true;
-      { ProfScope scope(ctx, PC_IPA_FOLD);
-        prf_fill(ctx, bv.seed, j0, R_BATCH_WEIGHT, 0, d_rho.get(), 1, 1, 1, K);
-        ctx->work[PC_IPA_FOLD] += (double)K * (r.M + 2);
-        launch(ctx, batch_weights_kernel, K, 128, 0, d_rho.get(), d_sc.get(), r.M, d_ab.get()); }
-      msm_run<Fq, Fp>(ctx, d_sc.get(), 0, d_pts.get(), 0, (int)N, 1, MsmConfig(), part.get());
-      { ProfScope scope(ctx, PC_MSM_REDUCE);
-        launch(ctx, batch_acc_kernel, 1, 1, 0, bv.acc.get(), part.get()); }
-      batch_g_scalars(ctx, bv.g.get(), d_us.get(), d_ab.get(), (int)C.k, K, K);
+      batch_fold(ctx, bv, j0, K, r.M, (int)C.k, d_pts.get(), d_sc.get(), d_us.get(), d_ab.get());
       ctx->sync();   // the batch may be used from another context (stream) next
       bv.broken = false;
     }
@@ -366,11 +448,32 @@ static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K
   bv.next += (uint64_t)K;
 }
 
-// 1 iff the weighted sum of every final check added is the identity: g through the SRS's fixed-base tables, plus acc
-static uint8_t batch_finalize(Ctx* ctx, const BatchVerifier& bv) {
+// The proofs of one tb_dev_batch_verifier_add (device memory): the device replay, then batch_fold, all enqueued without
+// waiting.  A proof the replay rejects clears bv.alive and adds nothing (its terms and g-term coefficients are 0).
+static void batch_add_dev(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len,
+                          const uint8_t* d_proofs, size_t proof_stride, size_t proof_len) {
+  const Shape& C = vk.shape;
+  const uint32_t j0 = (uint32_t)bv.next;
+  batch_claim(ctx, bv);
+  if (proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted: nothing is decoded
+  else {
+    bv.broken = true;
+    DevReplay r;
+    replay_batch_dev(ctx, vk, K, d_instance, instance_len, d_proofs, proof_stride, proof_len, r, bv.alive.get());
+    batch_fold(ctx, bv, j0, K, r.M, (int)C.k, r.pts.get(), r.sc.get(), r.us.get(), r.ab.get());
+    bv.pending = ctx;
+    bv.broken = false;
+  }
+  bv.next += (uint64_t)K;
+}
+
+// 1 iff no device replay rejected a proof and the weighted sum of every final check added is the identity: g through the
+// SRS's fixed-base tables, plus acc
+static uint8_t batch_finalize(Ctx* ctx, BatchVerifier& bv) {
+  batch_claim(ctx, bv);
   DevBuf<Xyzz<Fq>> acc_g(ctx, 1); DevBuf<uint8_t> d_ok(ctx, 1);
   bv.srs->commit_xyzz(ctx, false, bv.g.get(), (long long)bv.srs->n, 1, nullptr, 0, acc_g.get());
-  launch(ctx, verify_final_kernel, 1, 32, 0, bv.acc.get(), acc_g.get(), d_ok.get(), 1);
+  launch(ctx, verify_final_kernel, 1, 32, 0, bv.acc.get(), acc_g.get(), d_ok.get(), 1, (const uint8_t*)bv.alive.get());
   uint8_t ok = 0;
   d_ok.download(&ok, 1); ctx->sync();
   return ok;
@@ -405,6 +508,17 @@ static std::vector<Aff<Fq>> parse_commitments(const uint8_t* b, size_t cnt, cons
     out[i] = p;
   }
   return out;
+}
+
+// Refuses (TB_ERR_INVALID) a pointer that is not device memory of the context's device; nullptr entries are skipped
+static void require_device_memory(const Ctx& ctx, std::initializer_list<const void*> ptrs, const char* what) {
+  for (const void* p : ptrs) {
+    if (!p) continue;
+    cudaPointerAttributes a;
+    TB_CUDA(cudaPointerGetAttributes(&a, p));
+    TB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx.device,
+               std::string(what) + ": a buffer is not device memory of the context's device");
+  }
 }
 
 }  // namespace tb
@@ -460,6 +574,20 @@ tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proofs, c
   TB_API_END(ctx)
 }
 
+tb_status tb_dev_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proofs, const void* d_instance, const uint32_t* instance_len,
+                                 const void* d_proofs, size_t proof_stride, size_t proof_len, void* d_ok_out) {
+  TB_API_BEGIN(ctx)
+  const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
+  TB_REQUIRE(vk && n_proofs >= 1 && n_proofs <= 4096 && d_proofs && d_ok_out && proof_stride >= proof_len && (vk->shape.ni == 0 || (d_instance && instance_len)),
+             "tb_dev_verify_batch_vk arguments");
+  instance_total(vk->shape, instance_len);
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  require_device_memory(ctx->c, {d_proofs, d_ok_out, vk->shape.ni ? d_instance : nullptr}, "tb_dev_verify_batch_vk");
+  verify_batch_dev(&ctx->c, *vk, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len, static_cast<const uint8_t*>(d_proofs), proof_stride,
+                   proof_len, static_cast<uint8_t*>(d_ok_out));
+  TB_API_END(ctx)
+}
+
 tb_status tb_batch_verifier_create(tb_ctx* ctx, const tb_srs* srs_, const uint8_t seed[32], tb_batch_verifier** out) {
   TB_API_BEGIN(ctx)
   const Srs* srs = reinterpret_cast<const Srs*>(srs_);
@@ -472,6 +600,8 @@ tb_status tb_batch_verifier_create(tb_ctx* ctx, const tb_srs* srs_, const uint8_
   // zero bytes: the scalar 0 (Montgomery) and the XYZZ identity
   TB_CUDA(cudaMemsetAsync(bv->g.get(), 0, srs->n * sizeof(Fp), ctx->c.stream));
   TB_CUDA(cudaMemsetAsync(bv->acc.get(), 0, sizeof(Xyzz<Fq>), ctx->c.stream));
+  bv->alive = DevMem<uint8_t>(1);
+  TB_CUDA(cudaMemsetAsync(bv->alive.get(), 1, 1, ctx->c.stream));
   ctx->c.sync();
   *out = reinterpret_cast<tb_batch_verifier*>(bv.release());
   TB_API_END(ctx)
@@ -493,6 +623,27 @@ tb_status tb_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv_, const tb_vk
   instance_total(vk->shape, instance_len);
   TB_CUDA(cudaSetDevice(ctx->c.device));
   batch_add(&ctx->c, *bv, *vk, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len);
+  TB_API_END(ctx)
+}
+
+tb_status tb_dev_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv_, const tb_vk* vk_, uint32_t n_proofs, const void* d_instance,
+                                    const uint32_t* instance_len, const void* d_proofs, size_t proof_stride, size_t proof_len) {
+  TB_API_BEGIN(ctx)
+  BatchVerifier* bv = reinterpret_cast<BatchVerifier*>(bv_);
+  const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
+  // every refusal comes before the batch changes
+  TB_REQUIRE(bv && vk && n_proofs >= 1 && n_proofs <= 4096 && d_proofs && proof_stride >= proof_len && (vk->shape.ni == 0 || (d_instance && instance_len)),
+             "tb_dev_batch_verifier_add arguments");
+  TB_REQUIRE(!bv->finalized, "tb_dev_batch_verifier_add after tb_batch_verifier_finalize");
+  TB_REQUIRE(!bv->broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
+  TB_REQUIRE(vk->srs == bv->srs, "the verifying key refers to another SRS than the batch");
+  TB_REQUIRE(ctx->c.device == bv->device, "the context is on another device than the batch");
+  TB_REQUIRE(bv->next + n_proofs <= (1ull << 32), "a batch holds at most 2^32 proofs");
+  instance_total(vk->shape, instance_len);
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  require_device_memory(ctx->c, {d_proofs, vk->shape.ni ? d_instance : nullptr}, "tb_dev_batch_verifier_add");
+  batch_add_dev(&ctx->c, *bv, *vk, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len, static_cast<const uint8_t*>(d_proofs), proof_stride,
+                proof_len);
   TB_API_END(ctx)
 }
 

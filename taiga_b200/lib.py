@@ -49,6 +49,8 @@ _SIGS = {
     "tb_dev_from_mont": (_i, [_vp, _i, _vp, _sz]),
     "tb_dev_ntt": (_i, [_vp, _i, _u32, _i, _i, _u32, _vp, _vp, _vp]),
     "tb_dev_msm": (_i, [_vp, _i, _sz, _u32, _vp, _vp, _u32, _vp]),
+    "tb_dev_verify_batch_vk": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
+    "tb_dev_batch_verifier_add": (_i, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz]),
     "tb_srs_load": (_i, [_vp, _u32, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "tb_srs_free": (None, [_vp]),
     "tb_srs_commit": (_i, [_vp, _vp, _i, _u32, _vp, _vp, _vp]),
@@ -376,6 +378,33 @@ def _verify_batch(ctx, fn, h, instance, instance_len, proofs):
     return [bool(v) for v in ok]
 
 
+def _dev_proofs(proofs, proof_len):
+    """(B, address, stride, proof_len) of a CUDA uint8 tensor of B proof records, one per row (rows may be padded or be views
+    with any row stride); proof_len defaults to the row length."""
+    assert proofs.is_cuda and proofs.dtype.itemsize == 1 and proofs.dim() == 2 and proofs.stride(1) == 1
+    return proofs.shape[0], proofs.data_ptr(), proofs.stride(0), proofs.shape[1] if proof_len is None else int(proof_len)
+
+
+def _on_ctx_stream(ctx, *tensors):
+    """Orders the context's stream after the work torch has enqueued on its current stream (what made the tensors the next
+    call reads), and marks the tensors as used on the context's stream, so that torch's allocator does not hand their memory
+    out again before the call has run there."""
+    import torch
+    dev = tensors[0].device
+    s = torch.cuda.ExternalStream(ctx.stream, device=dev)
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(dev))
+    s.wait_event(ev)
+    for t in tensors:
+        if t is not None:
+            t.record_stream(s)
+
+
+def _dev_instance(instance):
+    assert instance is None or (instance.is_cuda and instance.dtype.itemsize == 1 and instance.is_contiguous())
+    return None if instance is None or instance.numel() == 0 else _vp(instance.data_ptr())
+
+
 class VerifyingKey:
     """The verifying key of one circuit (tb_vk): halo2's VerifyingKey<vesta::Affine> as Proof::verify uses it
     (proof.rs:45-54).  Holds the circuit's shape and the fixed / sigma commitments in host memory; refers to `srs`."""
@@ -395,6 +424,19 @@ class VerifyingKey:
     def verify_batch(self, instance, instance_len, proofs, ctx=None):
         """Proof::verify for a batch: proofs = list of byte strings; returns a list of booleans."""
         return _verify_batch(ctx or self.ctx, "tb_verify_batch_vk", self._h, instance, instance_len, proofs)
+
+    def verify_batch_dev(self, instance, instance_len, proofs, ok, ctx=None, proof_len=None):
+        """verify_batch over device memory, enqueued on the context's stream without waiting (tb_dev_verify_batch_vk):
+        `proofs` a CUDA uint8 tensor [B, >= proof_len] (one proof per row, any row stride), `instance` a contiguous CUDA
+        uint8 tensor of B * sum(instance_len) * 32 bytes, `ok` a CUDA uint8 tensor of B verdicts written in stream order.  The
+        context's stream first waits for torch's current stream, and the tensors are kept from reuse until it has run the call."""
+        ctx = ctx or self.ctx
+        B, addr, stride, plen = _dev_proofs(proofs, proof_len)
+        assert ok.is_cuda and ok.dtype.itemsize == 1 and ok.is_contiguous() and ok.numel() >= B
+        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+        _on_ctx_stream(ctx, proofs, instance, ok)
+        ctx._check(ctx._lib.tb_dev_verify_batch_vk(ctx._h, self._h, B, _dev_instance(instance), _ptr(lens), _vp(addr), stride, plen,
+                                                   _vp(ok.data_ptr())))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -423,8 +465,16 @@ class BatchVerifier:
 
     def add(self, vk, instance, instance_len, proofs, ctx=None):
         """add_proof for each of `proofs` (byte strings of one length, at most 4096) of vk's circuit; instance / instance_len
-        as in VerifyingKey.verify_batch.  A proof that fails before its final check makes finalize() False."""
+        as in VerifyingKey.verify_batch.  A proof that fails before its final check makes finalize() False.  With `proofs` a
+        CUDA tensor (and `instance` one, as in VerifyingKey.verify_batch_dev) the add runs on the device
+        (tb_dev_batch_verifier_add) and returns without waiting."""
         ctx = ctx or self.ctx
+        if hasattr(proofs, "is_cuda") and proofs.is_cuda:
+            B, addr, stride, plen = _dev_proofs(proofs, None)
+            lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+            _on_ctx_stream(ctx, proofs, instance)
+            ctx._check(ctx._lib.tb_dev_batch_verifier_add(ctx._h, self._h, vk._h, B, _dev_instance(instance), _ptr(lens), _vp(addr), stride, plen))
+            return
         B = len(proofs)
         plen = len(proofs[0]) if B else 0
         assert all(len(p) == plen for p in proofs)

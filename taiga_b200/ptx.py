@@ -148,9 +148,15 @@ class ProverService:
         circuits = [(vk, proofs, inst, lens, per) for vk, proofs, inst, lens, per in
                     zip(self.verifying_keys(), (c_proofs, v_proofs), (wit["c_inst"], wit["v_inst"]), (wit["c_len"], wit["v_len"]),
                         (COMPLIANCE_PER_PTX, VP_PER_PTX))]
+        import torch
+        dev = torch.device("cuda", self.srs.ctx.device)
+        # the bundle's proof records and instances go to the device once; the replay, the MSMs and the checks run there
+        on_dev = [(vk, torch.from_numpy(np.frombuffer(b"".join(proofs), np.uint8).reshape(len(proofs), -1).copy()).to(dev),
+                   torch.from_numpy(np.ascontiguousarray(inst, dtype=np.uint8).reshape(len(proofs), -1).copy()).to(dev), lens, per)
+                  for vk, proofs, inst, lens, per in circuits]
         bv = lib.BatchVerifier(self.srs, seed)
         try:
-            for vk, proofs, inst, lens, _ in circuits:
+            for vk, proofs, inst, lens, _ in on_dev:
                 for lo in range(0, len(proofs), max_batch):
                     bv.add(vk, inst[lo:lo + max_batch], lens, proofs[lo:lo + max_batch])
             if bv.finalize():
@@ -158,10 +164,13 @@ class ProverService:
         finally:
             bv.close()
         verdicts = [True] * n_ptx
-        for vk, proofs, inst, lens, per in circuits:
+        for vk, proofs, inst, lens, per in on_dev:
+            ok = torch.zeros(len(proofs), dtype=torch.uint8, device=dev)
             for lo in range(0, len(proofs), max_batch):
-                for i, ok in enumerate(vk.verify_batch(inst[lo:lo + max_batch], lens, proofs[lo:lo + max_batch]), lo):
-                    verdicts[i // per] &= ok
+                vk.verify_batch_dev(inst[lo:lo + max_batch], lens, proofs[lo:lo + max_batch], ok[lo:lo + max_batch])
+            self.srs.ctx.sync()
+            for i, v in enumerate(ok.tolist()):
+                verdicts[i // per] &= bool(v)
         return all(verdicts), verdicts
 
     @property

@@ -9,6 +9,9 @@ Reports, fastest of --repeats calls:
     time do not overlap);
   * the batch verifier (tb_batch_verifier): the same 384 proofs in one batch, both circuits, one finalize, with the same
     split into device MSMs and the rest;
+  * the device path (tb_dev_verify_batch_vk, and the batch verifier with device adds): proofs and instances already in device
+    memory, transcripts replayed on the device; wall time, and the device time of replay_kernel and of decompress_kernel
+    from torch.profiler (one profiled call);
   * the old path, which decoded every point on the host: the same points through the host build of the same decoder
     (tests/host_shim.cpp, g++ -O2, one thread), and the wall time that path would take (vk wall - device decode + host decode).
 
@@ -154,10 +157,50 @@ def main():
                 "batch_device_decode_weights_g_ms": round(bv_other_ms, 3), "batch_host_replay_and_copies_ms": round(bv_s * 1e3 - bv_msm_ms - bv_other_ms, 1)})
     print("tb_batch_verifier:  %d proofs in %.1f ms (%.0f proofs/s); device MSMs %.1f ms, device decode + weights + g-term %.2f ms, host replay and copies %.0f ms"
           % (n_proofs, bv_s * 1e3, n_proofs / bv_s, bv_msm_ms, bv_other_ms, bv_s * 1e3 - bv_msm_ms - bv_other_ms))
+    res.update(device_path(ctx, srs, vks, circuits, args.repeats, n_proofs))
     print("measured on: %s, power limit %s" % (res["gpu"], res["power_limit"]))
     print(json.dumps(res))
     for vk in vks:
         vk.close()
+
+
+def device_path(ctx, srs, vks, circuits, repeats, n_proofs):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    from taiga_b200 import lib
+    on_dev = [(vk, torch.from_numpy(np.frombuffer(b"".join(c[2]), np.uint8).reshape(len(c[2]), -1).copy()).cuda(),
+               torch.from_numpy(np.ascontiguousarray(c[3], dtype=np.uint8).reshape(len(c[2]), -1).copy()).cuda(), c[4]) for vk, c in zip(vks, circuits)]
+    oks = [torch.zeros(p.shape[0], dtype=torch.uint8, device="cuda") for _, p, _, _ in on_dev]
+    torch.cuda.synchronize()
+
+    def per_proof():
+        for (vk, p, i, lens), ok in zip(on_dev, oks):
+            vk.verify_batch_dev(i, lens, p, ok)
+        ctx.sync()
+        return [[bool(o.all())] for o in oks]
+
+    def batch():
+        bv = lib.BatchVerifier(srs, bytes(range(7, 39)))
+        for vk, p, i, lens in on_dev:
+            bv.add(vk, i, lens, p)
+        ok = bv.finalize()
+        bv.close()
+        return [[ok]]
+    out = {}
+    for name, fn in (("dev_vk", per_proof), ("dev_batch", batch)):
+        s = best(fn, repeats)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+        kern = {}
+        for e in prof.key_averages():
+            for k in ("replay_kernel", "decompress_kernel"):
+                if k in e.key:
+                    kern[k] = kern.get(k, 0.0) + e.device_time_total / 1e3
+        out.update({name + "_seconds": round(s, 4), name + "_proofs_per_s": round(n_proofs / s, 1),
+                    name + "_replay_kernel_ms": round(kern.get("replay_kernel", 0.0), 2), name + "_decompress_ms": round(kern.get("decompress_kernel", 0.0), 3)})
+        print("%-19s %d proofs in %.1f ms (%.0f proofs/s); replay_kernel %.2f ms, decompress_kernel %.3f ms of device time"
+              % (name + ":", n_proofs, s * 1e3, n_proofs / s, kern.get("replay_kernel", 0.0), kern.get("decompress_kernel", 0.0)))
+    return out
 
 
 def _gpu_name():
