@@ -183,56 +183,7 @@ static ReplayPlan replay_plan(const Shape& C) {
   return R;
 }
 
-// What the transcript replay of K proofs leaves for their final IPA checks.  Proof p's M variable-base terms are pts / sc at
-// [p * M, (p + 1) * M), the last two W and U with their scalars -f and -c*b*z; us[p] = the kk IPA challenges u_j and
-// ab[p] = (-c, -v), the coefficients of its g-term.  alive[p] = 0 for a proof rejected during the replay (a read that fails,
-// an identity absorbed, a non-canonical scalar or instance value, trailing bytes); its terms are the identity times 0, its ab 0.
-struct Replay {
-  int M = 0;
-  std::vector<Aff<Fq>> pts; std::vector<Fp> sc, us, ab; std::vector<char> alive;
-};
-
-// Replays, on the host, the transcripts of K proofs (host memory) of proof_len == C.proof_len bytes of the circuit of shape C,
-// whose fixed / sigma commitments are `vk_fixed` / `vk_sigma` (Montgomery).  Every point is decoded and every instance column
-// committed on the device first.
-static void replay_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
-                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, Replay& rep) {
-  const ReplayPlan plan = replay_plan(C);
-  const ReplayShape S = plan.bind(plan.blob.data());
-  const int kk = (int)C.k, ni = C.ni;
-  const size_t inst_total = instance_total(C, instance_len);
-  // ---- every point of the batch, decoded on the device: [K][npts]
-  const int npts = S.npts;
-  std::vector<Aff<Fq>> dec((size_t)K * npts);
-  std::vector<uint8_t> dec_ok((size_t)K * npts);
-  { DevBuf<uint8_t> d_proofs(ctx, (size_t)K * proof_len), d_ok(ctx, dec_ok.size()); DevBuf<uint32_t> d_off(ctx, npts); DevBuf<Aff<Fq>> d_pts(ctx, dec.size());
-    TB_CUDA(cudaMemcpy2DAsync(d_proofs.get(), proof_len, proofs, proof_stride, proof_len, K, cudaMemcpyHostToDevice, ctx->stream));
-    d_off.upload(C.point_offsets.data(), npts);
-    decompress(ctx, d_proofs.get(), proof_len, d_off.get(), npts, dec.size(), d_pts.get(), d_ok.get());
-    d_pts.download(dec.data(), dec.size()); d_ok.download(dec_ok.data(), dec_ok.size()); ctx->sync(); }
-  // ---- instance commitments for the whole batch: [K][ni]
-  std::vector<Aff<Fq>> inst_comm;
-  if (ni) {
-    DevBuf<Fp> iv(ctx, (size_t)K * ni * C.n);
-    upload_instance(ctx, C, K, instance, instance_len, iv.get());
-    inst_comm = commit_columns(ctx, srs, iv.get(), K * ni);
-  }
-  // ---- per proof: the shared replay
-  rep.M = S.M;
-  rep.pts.assign((size_t)K * rep.M, Aff<Fq>::inf());
-  rep.sc.assign((size_t)K * rep.M, Fp::zero()); rep.us.assign((size_t)K * kk, Fp::zero()); rep.ab.assign((size_t)K * 2, Fp::zero());
-  rep.alive.assign(K, 0);
-  std::vector<Fp> scratch(S.scratch);
-  for (int p = 0; p < K; ++p) {
-    const ReplayIn in = {proofs + (size_t)p * proof_stride, proof_len, dec.data() + (size_t)p * npts, dec_ok.data() + (size_t)p * npts,
-                         instance + 32 * inst_total * p, inst_total, ni ? inst_comm.data() + (size_t)p * ni : nullptr, vk_fixed.data(), vk_sigma.data(),
-                         srs.w_host, srs.u_host};
-    const ReplayOut out = {rep.pts.data() + (size_t)p * rep.M, rep.sc.data() + (size_t)p * rep.M, rep.us.data() + (size_t)p * kk, rep.ab.data() + 2 * p};
-    rep.alive[p] = replay_proof(S, in, scratch.data(), out) ? 1 : 0;
-  }
-}
-
-// One thread per proof: the shared replay over device memory.  A proof rejected during its replay gets alive[p] = 0 and, when
+// One thread per proof: replay_proof over device memory.  A proof rejected during its replay gets alive[p] = 0 and, when
 // batch_alive is given, sets *batch_alive = 0.
 constexpr int RP_THREADS = 32;
 __global__ void __launch_bounds__(RP_THREADS) replay_kernel(const ReplayShape S, int K, const uint8_t* __restrict__ proofs, size_t stride, size_t len,
@@ -251,81 +202,108 @@ __global__ void __launch_bounds__(RP_THREADS) replay_kernel(const ReplayShape S,
   if (!good && batch_alive) *batch_alive = 0;
 }
 
-// What the device replay of K proofs leaves, as Replay, on the device
+// What the transcript replay of K proofs leaves on the device for their final IPA checks.  Proof p's M variable-base terms
+// are pts / sc at [p * M, (p + 1) * M), the last two W and U with their scalars -f and -c*b*z; us[p] = the kk IPA challenges
+// u_j and ab[p] = (-c, -v), the coefficients of its g-term.  alive[p] = 0 for a proof rejected during the replay (a read that
+// fails, an identity absorbed, a non-canonical scalar or instance value, trailing bytes); its terms are the identity times 0,
+// its ab 0.
 struct DevReplay {
   int M = 0;
   DevBuf<Aff<Fq>> pts; DevBuf<Fp> sc, us, ab; DevBuf<uint8_t> alive;
 };
 
-// The replay of K proofs in device memory (proof p at d_proofs + p * proof_stride, proof_len == the shape's), enqueued on the
-// context's stream: the points decoded, the instance columns committed, then replay_kernel.  Nothing is waited for.
-static void replay_batch_dev(Ctx* ctx, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len, const uint8_t* d_proofs,
-                             size_t proof_stride, size_t proof_len, DevReplay& r, uint8_t* batch_alive) {
-  const Shape& C = vk.shape; const Srs& srs = *vk.srs;
-  const int ni = C.ni;
+// Replays the transcripts of K proofs of proof_len == C.proof_len bytes (proof p at proofs + p * proof_stride, in device
+// memory iff on_device) of the circuit of shape C, whose fixed / sigma commitments are `fixed` / `sigma` (Montgomery).
+// Every point is decoded and every instance column committed on the device first.  Proofs in host memory are copied to the
+// device for that, and are then replayed on the host after one wait, the results uploaded; proofs in device memory are
+// replayed by replay_kernel, enqueued without waiting, which also clears *batch_alive (when given) for a rejected proof.
+// Returns whether a host replay rejected a proof.
+static bool replay_batch(Ctx* ctx, bool on_device, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& fixed, const std::vector<Aff<Fq>>& sigma,
+                         int K, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len,
+                         DevReplay& r, uint8_t* batch_alive) {
+  const int kk = (int)C.k, ni = C.ni;
   const size_t inst_total = instance_total(C, instance_len);
-  // the shape's tables, the key's commitments and the point offsets: one upload
+  // the shape's tables, the point offsets and, for the device replay, the key's commitments: one upload
   ReplayPlan plan = replay_plan(C);
-  const Aff<Fq>* o_fixed = plan.put(vk.fixed); const Aff<Fq>* o_sigma = plan.put(vk.sigma); const uint32_t* o_off = plan.put(C.point_offsets);
+  const uint32_t* o_off = plan.put(C.point_offsets);
+  const Aff<Fq>* o_fixed = on_device ? plan.put(fixed) : nullptr; const Aff<Fq>* o_sigma = on_device ? plan.put(sigma) : nullptr;
   DevBuf<uint8_t> d_blob(ctx, plan.blob.size());
   d_blob.upload(plan.blob.data(), plan.blob.size());
-  const ReplayShape S = plan.bind(d_blob.get());
+  const ReplayShape S = plan.bind(on_device ? d_blob.get() : plan.blob.data());
   const int npts = S.npts;
+  // ---- every point of the batch, decoded on the device: [K][npts]
+  DevBuf<uint8_t> staged;
+  if (!on_device) {
+    staged = DevBuf<uint8_t>(ctx, (size_t)K * proof_len);
+    TB_CUDA(cudaMemcpy2DAsync(staged.get(), proof_len, proofs, proof_stride, proof_len, K, cudaMemcpyHostToDevice, ctx->stream));
+  }
   DevBuf<Aff<Fq>> dec(ctx, (size_t)K * npts); DevBuf<uint8_t> dec_ok(ctx, (size_t)K * npts);
-  decompress(ctx, d_proofs, proof_stride, ReplayPlan::at(d_blob.get(), o_off), npts, (size_t)K * npts, dec.get(), dec_ok.get());
+  decompress(ctx, on_device ? proofs : staged.get(), on_device ? proof_stride : proof_len, ReplayPlan::at(d_blob.get(), o_off), npts, (size_t)K * npts,
+             dec.get(), dec_ok.get());
+  // ---- instance commitments for the whole batch: [K][ni]
   DevBuf<Aff<Fq>> inst_comm(ctx, (size_t)K * ni);
   if (ni) {
     DevBuf<Fp> iv(ctx, (size_t)K * ni * C.n);
-    upload_instance(ctx, C, K, d_instance, instance_len, iv.get());
+    upload_instance(ctx, C, K, instance, instance_len, iv.get());
     commit_columns_dev(ctx, srs, iv.get(), K * ni, inst_comm.get());
   }
+  // ---- per proof: the shared replay
   r.M = S.M;
-  r.pts = DevBuf<Aff<Fq>>(ctx, (size_t)K * S.M); r.sc = DevBuf<Fp>(ctx, (size_t)K * S.M); r.us = DevBuf<Fp>(ctx, (size_t)K * C.k);
+  r.pts = DevBuf<Aff<Fq>>(ctx, (size_t)K * S.M); r.sc = DevBuf<Fp>(ctx, (size_t)K * S.M); r.us = DevBuf<Fp>(ctx, (size_t)K * kk);
   r.ab = DevBuf<Fp>(ctx, (size_t)K * 2); r.alive = DevBuf<uint8_t>(ctx, K);
-  DevBuf<Fp> scratch(ctx, (size_t)K * S.scratch);
-  ProfScope scope(ctx, PC_TRANSCRIPT);
-  launch(ctx, replay_kernel, (unsigned)((K + RP_THREADS - 1) / RP_THREADS), RP_THREADS, 0, S, K, d_proofs, proof_stride, proof_len, d_instance, inst_total,
-         dec.get(), dec_ok.get(), inst_comm.get(), ReplayPlan::at(d_blob.get(), o_fixed), ReplayPlan::at(d_blob.get(), o_sigma), srs.wu.get(), scratch.get(),
-         r.pts.get(), r.sc.get(), r.us.get(), r.ab.get(), r.alive.get(), batch_alive);
+  if (on_device) {
+    DevBuf<Fp> scratch(ctx, (size_t)K * S.scratch);
+    ProfScope scope(ctx, PC_TRANSCRIPT);
+    launch(ctx, replay_kernel, (unsigned)((K + RP_THREADS - 1) / RP_THREADS), RP_THREADS, 0, S, K, proofs, proof_stride, proof_len, instance, inst_total,
+           dec.get(), dec_ok.get(), inst_comm.get(), ReplayPlan::at(d_blob.get(), o_fixed), ReplayPlan::at(d_blob.get(), o_sigma), srs.wu.get(), scratch.get(),
+           r.pts.get(), r.sc.get(), r.us.get(), r.ab.get(), r.alive.get(), batch_alive);
+    return false;
+  }
+  std::vector<Aff<Fq>> h_dec(dec.n), h_inst(inst_comm.n); std::vector<uint8_t> h_ok(dec_ok.n);
+  dec.download(h_dec.data(), h_dec.size()); dec_ok.download(h_ok.data(), h_ok.size());
+  if (ni) inst_comm.download(h_inst.data(), h_inst.size());
+  ctx->sync();
+  std::vector<Aff<Fq>> pts((size_t)K * S.M, Aff<Fq>::inf());
+  std::vector<Fp> sc((size_t)K * S.M, Fp::zero()), us((size_t)K * kk, Fp::zero()), ab((size_t)K * 2, Fp::zero()), scratch(S.scratch);
+  std::vector<uint8_t> alive(K);
+  for (int p = 0; p < K; ++p) {
+    const ReplayIn in = {proofs + (size_t)p * proof_stride, proof_len, h_dec.data() + (size_t)p * npts, h_ok.data() + (size_t)p * npts,
+                         instance + 32 * inst_total * p, inst_total, h_inst.data() + (size_t)p * ni, fixed.data(), sigma.data(), srs.w_host, srs.u_host};
+    const ReplayOut out = {pts.data() + (size_t)p * S.M, sc.data() + (size_t)p * S.M, us.data() + (size_t)p * kk, ab.data() + 2 * p};
+    alive[p] = replay_proof(S, in, scratch.data(), out) ? 1 : 0;
+  }
+  r.pts.upload(pts.data(), pts.size()); r.sc.upload(sc.data(), sc.size()); r.us.upload(us.data(), us.size()); r.ab.upload(ab.data(), ab.size());
+  r.alive.upload(alive.data(), K);
+  return std::find(alive.begin(), alive.end(), 0) != alive.end();
 }
 
-// n_proofs proofs of the circuit of shape C, each checked on its own: the replay, then both MSMs of every proof's final
-// check for the whole batch on the device (each proof its own g-term), then the identity test
-static void verify_batch(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& vk_fixed, const std::vector<Aff<Fq>>& vk_sigma, int K,
-                         const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
+// K proofs of the circuit of shape C, each checked on its own: the replay, then both MSMs of every proof's final check for
+// the whole batch on the device (each proof its own g-term), then the identity test.  d_ok[p] = 1 iff proof p passes its
+// replay and its check; written in stream order.
+static void verify_batch(Ctx* ctx, bool on_device, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& fixed, const std::vector<Aff<Fq>>& sigma,
+                         int K, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len,
+                         uint8_t* d_ok) {
   const size_t n = C.n;
-  instance_total(C, instance_len);
-  for (int p = 0; p < K; ++p) ok_out[p] = 0;
-  if (proof_len != C.proof_len) return;   // no proof of this length is accepted
-  Replay r;
-  replay_batch(ctx, C, srs, vk_fixed, vk_sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r);
-  DevBuf<Aff<Fq>> d_pts(ctx, r.pts.size()); DevBuf<Fp> d_sc(ctx, r.sc.size()), d_us(ctx, r.us.size()), d_ab(ctx, r.ab.size()), d_gs(ctx, (size_t)K * n);
-  DevBuf<Xyzz<Fq>> acc_v(ctx, K), acc_g(ctx, K); DevBuf<uint8_t> d_ok(ctx, K);
-  d_pts.upload(r.pts.data(), r.pts.size()); d_sc.upload(r.sc.data(), r.sc.size()); d_us.upload(r.us.data(), r.us.size()); d_ab.upload(r.ab.data(), r.ab.size());
-  d_gs.zero();
-  msm_run<Fq, Fp>(ctx, d_sc.get(), r.M, d_pts.get(), r.M, r.M, K, MsmConfig(), acc_v.get());
-  batch_g_scalars(ctx, d_gs.get(), d_us.get(), d_ab.get(), (int)C.k, K, 1);
-  srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
-  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok.get(), K, (const uint8_t*)nullptr);
-  std::vector<uint8_t> hok(K);
-  d_ok.download(hok.data(), K); ctx->sync();
-  for (int p = 0; p < K; ++p) ok_out[p] = (r.alive[p] && hok[p]) ? 1 : 0;
-}
-
-// The same for proofs, instance values and verdicts in device memory, enqueued on the context's stream without waiting:
-// d_ok_out[p] = 1 iff proof p is accepted.  A proof_len other than the shape's gives 0 for every proof, nothing decoded.
-static void verify_batch_dev(Ctx* ctx, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len, const uint8_t* d_proofs,
-                             size_t proof_stride, size_t proof_len, uint8_t* d_ok_out) {
-  const Shape& C = vk.shape; const size_t n = C.n;
-  if (proof_len != C.proof_len) { TB_CUDA(cudaMemsetAsync(d_ok_out, 0, K, ctx->stream)); return; }
   DevReplay r;
-  replay_batch_dev(ctx, vk, K, d_instance, instance_len, d_proofs, proof_stride, proof_len, r, nullptr);
+  replay_batch(ctx, on_device, C, srs, fixed, sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r, nullptr);
   DevBuf<Fp> d_gs(ctx, (size_t)K * n); DevBuf<Xyzz<Fq>> acc_v(ctx, K), acc_g(ctx, K);
   d_gs.zero();
   msm_run<Fq, Fp>(ctx, r.sc.get(), r.M, r.pts.get(), r.M, r.M, K, MsmConfig(), acc_v.get());
   batch_g_scalars(ctx, d_gs.get(), r.us.get(), r.ab.get(), (int)C.k, K, 1);
-  vk.srs->commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
-  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok_out, K, (const uint8_t*)r.alive.get());
+  srs.commit_xyzz(ctx, false, d_gs.get(), (long long)n, K, nullptr, 0, acc_g.get());
+  launch(ctx, verify_final_kernel, (K + 31) / 32, 32, 0, acc_v.get(), acc_g.get(), d_ok, K, (const uint8_t*)r.alive.get());
+}
+
+// The same for proofs in host memory, waited for: the verdicts at ok_out on the host.  A proof_len other than the shape's
+// gives 0 for every proof, nothing decoded.
+static void verify_batch_host(Ctx* ctx, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& fixed, const std::vector<Aff<Fq>>& sigma, int K,
+                              const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs, size_t proof_stride, size_t proof_len,
+                              uint8_t* ok_out) {
+  memset(ok_out, 0, K);
+  if (proof_len != C.proof_len) return;   // no proof of this length is accepted
+  DevBuf<uint8_t> d_ok(ctx, K);
+  verify_batch(ctx, false, C, srs, fixed, sigma, K, instance, instance_len, proofs, proof_stride, proof_len, d_ok.get());
+  d_ok.download(ok_out, K); ctx->sync();
 }
 
 // ---------------------------------------------------------------- batch verifier (tb_batch_verifier)
@@ -424,45 +402,28 @@ static void batch_fold(Ctx* ctx, BatchVerifier& bv, uint32_t j0, int K, int M, i
   batch_g_scalars(ctx, bv.g.get(), us, ab, kk, K, K);
 }
 
-// The proofs of one tb_batch_verifier_add: replay on the host, then (unless a proof was rejected) batch_fold
-static void batch_add(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K, const uint8_t* instance, const uint32_t* instance_len,
-                      const uint8_t* proofs, size_t proof_stride, size_t proof_len) {
-  const Shape& C = vk.shape;
-  const uint32_t j0 = (uint32_t)bv.next;
-  batch_claim(ctx, bv);
-  if (!bv.rejected && proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted
-  if (!bv.rejected) {
-    Replay r;
-    replay_batch(ctx, C, *vk.srs, vk.fixed, vk.sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r);
-    if (std::find(r.alive.begin(), r.alive.end(), 0) != r.alive.end()) bv.rejected = true;
-    else {
-      const size_t N = (size_t)K * r.M;
-      DevBuf<Aff<Fq>> d_pts(ctx, N); DevBuf<Fp> d_sc(ctx, N), d_us(ctx, r.us.size()), d_ab(ctx, r.ab.size());
-      d_pts.upload(r.pts.data(), N); d_sc.upload(r.sc.data(), N); d_us.upload(r.us.data(), r.us.size()); d_ab.upload(r.ab.data(), r.ab.size());
-      bv.broken = true;
-      batch_fold(ctx, bv, j0, K, r.M, (int)C.k, d_pts.get(), d_sc.get(), d_us.get(), d_ab.get());
-      ctx->sync();   // the batch may be used from another context (stream) next
-      bv.broken = false;
-    }
-  }
-  bv.next += (uint64_t)K;
-}
-
-// The proofs of one tb_dev_batch_verifier_add (device memory): the device replay, then batch_fold, all enqueued without
-// waiting.  A proof the replay rejects clears bv.alive and adds nothing (its terms and g-term coefficients are 0).
-static void batch_add_dev(Ctx* ctx, BatchVerifier& bv, const VerifyingKey& vk, int K, const uint8_t* d_instance, const uint32_t* instance_len,
-                          const uint8_t* d_proofs, size_t proof_stride, size_t proof_len) {
-  const Shape& C = vk.shape;
+// The proofs of one tb_batch_verifier_add (host memory) or tb_dev_batch_verifier_add (device memory): the replay, then
+// batch_fold.  A host add does nothing once a proof was rejected, folds nothing when its replay rejects a proof, and waits
+// for its work.  A device add folds every proof (a rejected one clears bv.alive and adds nothing: its terms and g-term
+// coefficients are 0) and returns without waiting.
+static void batch_add(Ctx* ctx, bool on_device, BatchVerifier& bv, const Shape& C, const Srs& srs, const std::vector<Aff<Fq>>& fixed,
+                      const std::vector<Aff<Fq>>& sigma, int K, const uint8_t* instance, const uint32_t* instance_len, const uint8_t* proofs,
+                      size_t proof_stride, size_t proof_len) {
   const uint32_t j0 = (uint32_t)bv.next;
   batch_claim(ctx, bv);
   if (proof_len != C.proof_len) bv.rejected = true;   // no proof of this length is accepted: nothing is decoded
-  else {
-    bv.broken = true;
+  else if (on_device || !bv.rejected) {
+    bv.broken = on_device;   // the device replay writes bv.alive
     DevReplay r;
-    replay_batch_dev(ctx, vk, K, d_instance, instance_len, d_proofs, proof_stride, proof_len, r, bv.alive.get());
-    batch_fold(ctx, bv, j0, K, r.M, (int)C.k, r.pts.get(), r.sc.get(), r.us.get(), r.ab.get());
-    bv.pending = ctx;
-    bv.broken = false;
+    if (replay_batch(ctx, on_device, C, srs, fixed, sigma, K, instance, instance_len, proofs, proof_stride, proof_len, r, on_device ? bv.alive.get() : nullptr))
+      bv.rejected = true;
+    else {
+      bv.broken = true;
+      batch_fold(ctx, bv, j0, K, r.M, (int)C.k, r.pts.get(), r.sc.get(), r.us.get(), r.ab.get());
+      if (on_device) bv.pending = ctx;
+      else ctx->sync();   // the batch may be used from another context (stream) next
+      bv.broken = false;
+    }
   }
   bv.next += (uint64_t)K;
 }
@@ -521,6 +482,25 @@ static void require_device_memory(const Ctx& ctx, std::initializer_list<const vo
   }
 }
 
+// Refuses (TB_ERR_INVALID, "<what> arguments") a verifier call of no proofs or more than 4096, without proofs, with rows
+// shorter than proof_len or without the instance values of a circuit that has instance columns; and what instance_total
+// refuses.  Every verifier entry point checks this before it changes or launches anything.
+static void require_proofs(const Shape& C, uint32_t n_proofs, const void* instance, const uint32_t* instance_len, const void* proofs, size_t proof_stride,
+                           size_t proof_len, const char* what) {
+  TB_REQUIRE(n_proofs >= 1 && n_proofs <= 4096 && proofs && proof_stride >= proof_len && (C.ni == 0 || (instance && instance_len)),
+             std::string(what) + " arguments");
+  instance_total(C, instance_len);
+}
+
+// Refuses (TB_ERR_INVALID) an add of n_proofs proofs over `srs` on `ctx` that the batch cannot take, before the batch changes
+static void require_batch(const Ctx& ctx, const BatchVerifier& bv, const Srs* srs, uint32_t n_proofs, const char* what) {
+  TB_REQUIRE(!bv.finalized, std::string(what) + " after tb_batch_verifier_finalize");
+  TB_REQUIRE(!bv.broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
+  TB_REQUIRE(srs == bv.srs, "the verifying key refers to another SRS than the batch");
+  TB_REQUIRE(ctx.device == bv.device, "the context is on another device than the batch");
+  TB_REQUIRE(bv.next + n_proofs <= (1ull << 32), "a batch holds at most 2^32 proofs");
+}
+
 }  // namespace tb
 
 using namespace tb;
@@ -530,10 +510,11 @@ tb_status tb_verify_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const
                           size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
   TB_API_BEGIN(ctx)
   const Circuit* C = reinterpret_cast<const Circuit*>(pk);
-  TB_REQUIRE(C && n_proofs >= 1 && n_proofs <= 4096 && proofs && ok_out && proof_stride >= proof_len && (C->ni == 0 || (instance && instance_len)), "tb_verify_batch arguments");
+  TB_REQUIRE(C && ok_out, "tb_verify_batch arguments");
+  require_proofs(*C, n_proofs, instance, instance_len, proofs, proof_stride, proof_len, "tb_verify_batch");
   TB_CUDA(cudaSetDevice(ctx->c.device));
   pk_commitments(&ctx->c, *C);
-  verify_batch(&ctx->c, *C, *C->srs, C->vk_fixed, C->vk_sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
+  verify_batch_host(&ctx->c, *C, *C->srs, C->vk_fixed, C->vk_sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
   TB_API_END(ctx)
 }
 
@@ -567,10 +548,10 @@ tb_status tb_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proofs, c
                              size_t proof_stride, size_t proof_len, uint8_t* ok_out) {
   TB_API_BEGIN(ctx)
   const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
-  TB_REQUIRE(vk && n_proofs >= 1 && n_proofs <= 4096 && proofs && ok_out && proof_stride >= proof_len && (vk->shape.ni == 0 || (instance && instance_len)),
-             "tb_verify_batch_vk arguments");
+  TB_REQUIRE(vk && ok_out, "tb_verify_batch_vk arguments");
+  require_proofs(vk->shape, n_proofs, instance, instance_len, proofs, proof_stride, proof_len, "tb_verify_batch_vk");
   TB_CUDA(cudaSetDevice(ctx->c.device));
-  verify_batch(&ctx->c, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
+  verify_batch_host(&ctx->c, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len, ok_out);
   TB_API_END(ctx)
 }
 
@@ -578,13 +559,15 @@ tb_status tb_dev_verify_batch_vk(tb_ctx* ctx, const tb_vk* vk_, uint32_t n_proof
                                  const void* d_proofs, size_t proof_stride, size_t proof_len, void* d_ok_out) {
   TB_API_BEGIN(ctx)
   const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
-  TB_REQUIRE(vk && n_proofs >= 1 && n_proofs <= 4096 && d_proofs && d_ok_out && proof_stride >= proof_len && (vk->shape.ni == 0 || (d_instance && instance_len)),
-             "tb_dev_verify_batch_vk arguments");
-  instance_total(vk->shape, instance_len);
+  TB_REQUIRE(vk && d_ok_out, "tb_dev_verify_batch_vk arguments");
+  require_proofs(vk->shape, n_proofs, d_instance, instance_len, d_proofs, proof_stride, proof_len, "tb_dev_verify_batch_vk");
   TB_CUDA(cudaSetDevice(ctx->c.device));
   require_device_memory(ctx->c, {d_proofs, d_ok_out, vk->shape.ni ? d_instance : nullptr}, "tb_dev_verify_batch_vk");
-  verify_batch_dev(&ctx->c, *vk, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len, static_cast<const uint8_t*>(d_proofs), proof_stride,
-                   proof_len, static_cast<uint8_t*>(d_ok_out));
+  if (proof_len != vk->shape.proof_len)   // no proof of this length is accepted: nothing is decoded
+    TB_CUDA(cudaMemsetAsync(d_ok_out, 0, n_proofs, ctx->c.stream));
+  else
+    verify_batch(&ctx->c, true, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len,
+                 static_cast<const uint8_t*>(d_proofs), proof_stride, proof_len, static_cast<uint8_t*>(d_ok_out));
   TB_API_END(ctx)
 }
 
@@ -612,17 +595,11 @@ tb_status tb_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv_, const tb_vk
   TB_API_BEGIN(ctx)
   BatchVerifier* bv = reinterpret_cast<BatchVerifier*>(bv_);
   const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
-  // every refusal comes before the batch changes
-  TB_REQUIRE(bv && vk && n_proofs >= 1 && n_proofs <= 4096 && proofs && proof_stride >= proof_len && (vk->shape.ni == 0 || (instance && instance_len)),
-             "tb_batch_verifier_add arguments");
-  TB_REQUIRE(!bv->finalized, "tb_batch_verifier_add after tb_batch_verifier_finalize");
-  TB_REQUIRE(!bv->broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
-  TB_REQUIRE(vk->srs == bv->srs, "the verifying key refers to another SRS than the batch");
-  TB_REQUIRE(ctx->c.device == bv->device, "the context is on another device than the batch");
-  TB_REQUIRE(bv->next + n_proofs <= (1ull << 32), "a batch holds at most 2^32 proofs");
-  instance_total(vk->shape, instance_len);
+  TB_REQUIRE(bv && vk, "tb_batch_verifier_add arguments");
+  require_proofs(vk->shape, n_proofs, instance, instance_len, proofs, proof_stride, proof_len, "tb_batch_verifier_add");
+  require_batch(ctx->c, *bv, vk->srs, n_proofs, "tb_batch_verifier_add");
   TB_CUDA(cudaSetDevice(ctx->c.device));
-  batch_add(&ctx->c, *bv, *vk, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len);
+  batch_add(&ctx->c, false, *bv, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, instance, instance_len, proofs, proof_stride, proof_len);
   TB_API_END(ctx)
 }
 
@@ -631,19 +608,13 @@ tb_status tb_dev_batch_verifier_add(tb_ctx* ctx, tb_batch_verifier* bv_, const t
   TB_API_BEGIN(ctx)
   BatchVerifier* bv = reinterpret_cast<BatchVerifier*>(bv_);
   const VerifyingKey* vk = reinterpret_cast<const VerifyingKey*>(vk_);
-  // every refusal comes before the batch changes
-  TB_REQUIRE(bv && vk && n_proofs >= 1 && n_proofs <= 4096 && d_proofs && proof_stride >= proof_len && (vk->shape.ni == 0 || (d_instance && instance_len)),
-             "tb_dev_batch_verifier_add arguments");
-  TB_REQUIRE(!bv->finalized, "tb_dev_batch_verifier_add after tb_batch_verifier_finalize");
-  TB_REQUIRE(!bv->broken, "an earlier tb_batch_verifier_add failed part way: the batch can only be freed");
-  TB_REQUIRE(vk->srs == bv->srs, "the verifying key refers to another SRS than the batch");
-  TB_REQUIRE(ctx->c.device == bv->device, "the context is on another device than the batch");
-  TB_REQUIRE(bv->next + n_proofs <= (1ull << 32), "a batch holds at most 2^32 proofs");
-  instance_total(vk->shape, instance_len);
+  TB_REQUIRE(bv && vk, "tb_dev_batch_verifier_add arguments");
+  require_proofs(vk->shape, n_proofs, d_instance, instance_len, d_proofs, proof_stride, proof_len, "tb_dev_batch_verifier_add");
+  require_batch(ctx->c, *bv, vk->srs, n_proofs, "tb_dev_batch_verifier_add");
   TB_CUDA(cudaSetDevice(ctx->c.device));
   require_device_memory(ctx->c, {d_proofs, vk->shape.ni ? d_instance : nullptr}, "tb_dev_batch_verifier_add");
-  batch_add_dev(&ctx->c, *bv, *vk, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len, static_cast<const uint8_t*>(d_proofs), proof_stride,
-                proof_len);
+  batch_add(&ctx->c, true, *bv, vk->shape, *vk->srs, vk->fixed, vk->sigma, (int)n_proofs, static_cast<const uint8_t*>(d_instance), instance_len,
+            static_cast<const uint8_t*>(d_proofs), proof_stride, proof_len);
   TB_API_END(ctx)
 }
 

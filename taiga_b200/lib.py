@@ -366,43 +366,43 @@ class ProvingKey:
             pass
 
 
-def _verify_batch(ctx, fn, h, instance, instance_len, proofs):
+def _host_args(instance, instance_len, proofs):
+    """(n_proofs, instance, instance_len, proofs, proof_stride, proof_len) of a verifier call on host memory: `proofs` byte
+    strings of one length, packed one after the other."""
     B = len(proofs)
-    plen = len(proofs[0])
+    plen = len(proofs[0]) if B else 0
     assert all(len(p) == plen for p in proofs)
-    buf = np.frombuffer(b"".join(proofs), np.uint8).copy()
-    inst = _u8(instance)
-    lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
+    buf = np.frombuffer(b"".join(proofs), np.uint8).copy() if B else np.zeros(1, np.uint8)
+    return B, _u8(instance), np.ascontiguousarray(instance_len, dtype=np.uint32), buf, plen, plen
+
+
+def _verify_batch(ctx, fn, h, instance, instance_len, proofs):
+    B, inst, lens, buf, stride, plen = _host_args(instance, instance_len, proofs)
     ok = np.zeros(B, np.uint8)
-    ctx._check(getattr(ctx._lib, fn)(ctx._h, h, B, _ptr(inst), _ptr(lens), _ptr(buf), plen, plen, _ptr(ok)))
+    ctx._check(getattr(ctx._lib, fn)(ctx._h, h, B, _ptr(inst), _ptr(lens), _ptr(buf), stride, plen, _ptr(ok)))
     return [bool(v) for v in ok]
 
 
-def _dev_proofs(proofs, proof_len):
-    """(B, address, stride, proof_len) of a CUDA uint8 tensor of B proof records, one per row (rows may be padded or be views
-    with any row stride); proof_len defaults to the row length."""
-    assert proofs.is_cuda and proofs.dtype.itemsize == 1 and proofs.dim() == 2 and proofs.stride(1) == 1
-    return proofs.shape[0], proofs.data_ptr(), proofs.stride(0), proofs.shape[1] if proof_len is None else int(proof_len)
-
-
-def _on_ctx_stream(ctx, *tensors):
-    """Orders the context's stream after the work torch has enqueued on its current stream (what made the tensors the next
-    call reads), and marks the tensors as used on the context's stream, so that torch's allocator does not hand their memory
-    out again before the call has run there."""
+def _dev_args(ctx, instance, instance_len, proofs, proof_len, *tensors):
+    """(n_proofs, instance, instance_len, proofs, proof_stride, proof_len) of a verifier call on device memory: `proofs` a
+    CUDA uint8 tensor of B proof records, one per row (rows may be padded or be views with any row stride; proof_len defaults
+    to the row length), `instance` a contiguous CUDA uint8 tensor or None.  Orders the context's stream after the work torch
+    has enqueued on its current stream (what made the tensors the call reads), and marks `proofs`, `instance` and `tensors` as
+    used on the context's stream, so that torch's allocator does not hand their memory out again before the call has run there."""
     import torch
-    dev = tensors[0].device
+    assert proofs.is_cuda and proofs.dtype.itemsize == 1 and proofs.dim() == 2 and proofs.stride(1) == 1
+    assert instance is None or (instance.is_cuda and instance.dtype.itemsize == 1 and instance.is_contiguous())
+    dev = proofs.device
     s = torch.cuda.ExternalStream(ctx.stream, device=dev)
     ev = torch.cuda.Event()
     ev.record(torch.cuda.current_stream(dev))
     s.wait_event(ev)
-    for t in tensors:
+    for t in (proofs, instance) + tensors:
         if t is not None:
             t.record_stream(s)
-
-
-def _dev_instance(instance):
-    assert instance is None or (instance.is_cuda and instance.dtype.itemsize == 1 and instance.is_contiguous())
-    return None if instance is None or instance.numel() == 0 else _vp(instance.data_ptr())
+    inst = None if instance is None or instance.numel() == 0 else _vp(instance.data_ptr())
+    return (proofs.shape[0], inst, np.ascontiguousarray(instance_len, dtype=np.uint32), _vp(proofs.data_ptr()), proofs.stride(0),
+            proofs.shape[1] if proof_len is None else int(proof_len))
 
 
 class VerifyingKey:
@@ -431,12 +431,9 @@ class VerifyingKey:
         uint8 tensor of B * sum(instance_len) * 32 bytes, `ok` a CUDA uint8 tensor of B verdicts written in stream order.  The
         context's stream first waits for torch's current stream, and the tensors are kept from reuse until it has run the call."""
         ctx = ctx or self.ctx
-        B, addr, stride, plen = _dev_proofs(proofs, proof_len)
-        assert ok.is_cuda and ok.dtype.itemsize == 1 and ok.is_contiguous() and ok.numel() >= B
-        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
-        _on_ctx_stream(ctx, proofs, instance, ok)
-        ctx._check(ctx._lib.tb_dev_verify_batch_vk(ctx._h, self._h, B, _dev_instance(instance), _ptr(lens), _vp(addr), stride, plen,
-                                                   _vp(ok.data_ptr())))
+        assert ok.is_cuda and ok.dtype.itemsize == 1 and ok.is_contiguous() and ok.numel() >= proofs.shape[0]
+        B, inst, lens, addr, stride, plen = _dev_args(ctx, instance, instance_len, proofs, proof_len, ok)
+        ctx._check(ctx._lib.tb_dev_verify_batch_vk(ctx._h, self._h, B, inst, _ptr(lens), addr, stride, plen, _vp(ok.data_ptr())))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -470,18 +467,11 @@ class BatchVerifier:
         (tb_dev_batch_verifier_add) and returns without waiting."""
         ctx = ctx or self.ctx
         if hasattr(proofs, "is_cuda") and proofs.is_cuda:
-            B, addr, stride, plen = _dev_proofs(proofs, None)
-            lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
-            _on_ctx_stream(ctx, proofs, instance)
-            ctx._check(ctx._lib.tb_dev_batch_verifier_add(ctx._h, self._h, vk._h, B, _dev_instance(instance), _ptr(lens), _vp(addr), stride, plen))
-            return
-        B = len(proofs)
-        plen = len(proofs[0]) if B else 0
-        assert all(len(p) == plen for p in proofs)
-        buf = np.frombuffer(b"".join(proofs), np.uint8).copy() if B else np.zeros(1, np.uint8)
-        inst = _u8(instance)
-        lens = np.ascontiguousarray(instance_len, dtype=np.uint32)
-        ctx._check(ctx._lib.tb_batch_verifier_add(ctx._h, self._h, vk._h, B, _ptr(inst), _ptr(lens), _ptr(buf), plen, plen))
+            B, inst, lens, addr, stride, plen = _dev_args(ctx, instance, instance_len, proofs, None)
+            ctx._check(ctx._lib.tb_dev_batch_verifier_add(ctx._h, self._h, vk._h, B, inst, _ptr(lens), addr, stride, plen))
+        else:
+            B, inst, lens, buf, stride, plen = _host_args(instance, instance_len, proofs)
+            ctx._check(ctx._lib.tb_batch_verifier_add(ctx._h, self._h, vk._h, B, _ptr(inst), _ptr(lens), _ptr(buf), stride, plen))
 
     def finalize(self, ctx=None):
         """True iff every proof added would be accepted by VerifyingKey.verify_batch.  Consumes the batch."""
