@@ -158,6 +158,23 @@ tb_status tb_pk_commitments(tb_ctx* ctx, const tb_pk* pk, uint8_t* fixed_commitm
 tb_status tb_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const uint8_t* advice, const uint8_t* instance,
                          const uint32_t* instance_len, const uint8_t seed[32], uint32_t first_proof_index, uint8_t* proofs_out,
                          size_t proof_stride);
+/* Proving into device memory (proofs that go on to tb_dev_verify_batch_vk, a device batch verifier or a collective without
+ * crossing the host): tb_prove_batch with d_advice, d_instance (when the circuit has instance columns), d_proofs_out and
+ * d_status_out in device memory of the context's device, in the layouts and encodings of tb_prove_batch; instance_len and seed
+ * are host arrays.  Any proof_stride >= tb_pk_proof_len is allowed, odd ones included.  The call enqueues all its work on the
+ * context's stream and returns without waiting; the caller keeps every buffer alive and unmodified, and the key unfreed (or
+ * frees it, which waits for the device), until the stream has passed the call.  Written in stream order, per proof i:
+ *   d_status_out[i] = TB_PROVED            record i holds the bytes tb_prove_batch writes for (seed, first_proof_index + i)
+ *                   = 1 + l                an input of lookup l (the lowest such l) is not in its table (ConstraintSystemFailure)
+ *                   = TB_PROVE_INTERNAL    the transcript reports an error (tb_prove_batch's TB_ERR_INTERNAL)
+ * A record whose status is not TB_PROVED is all zero bytes, which no verifier accepts; the bytes between records are not
+ * written.  A proof's status and record do not depend on the other proofs of the call.  The call refuses (TB_ERR_INVALID,
+ * nothing enqueued, outputs untouched) what tb_prove_batch refuses, a null d_status_out, and a buffer that is not device
+ * memory of the context's device. */
+enum { TB_PROVED = 0, TB_PROVE_INTERNAL = 0xFFFFFFFFu };
+tb_status tb_dev_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const void* d_advice, const void* d_instance,
+                             const uint32_t* instance_len, const uint8_t seed[32], uint32_t first_proof_index,
+                             void* d_proofs_out, size_t proof_stride, uint32_t* d_status_out);
 
 /* ---- witness check: MockProver::run(k, circuit, instance).verify() for n_proofs witnesses of one circuit, without proving
  * (the check of transparent execution, verify_transparently; taiga_halo2/src/circuit/resource_logic_circuit.rs).

@@ -264,6 +264,20 @@ class Proof {
     return out;
   }
 
+  // create_batch into device memory of the context's device (tb_dev_prove_batch): n advice tables at d_advice, the instance
+  // values of each proof (canonical bytes, columns concatenated) at d_instance, proof i written at d_proofs + i * proof_stride
+  // and its status at d_status[i] (TB_PROVED, 1 + l for a lookup l input outside its table, TB_PROVE_INTERNAL; a record whose
+  // status is not TB_PROVED is zeros).  Returns without waiting: read the status from d_status after the context's stream has
+  // passed the call.  Throws Error for a refused call (nothing is enqueued).  The seed rules of create apply.
+  static void create_batch_device(const ProvingKey& pk, const Params& params, uint32_t n, const void* d_advice, const void* d_instance,
+                                  const std::vector<uint32_t>& instance_len, const std::array<uint8_t, 32>& rng_seed, uint32_t first_proof_index,
+                                  void* d_proofs, size_t proof_stride, uint32_t* d_status) {
+    if (&pk.params() != &params) throw Error(TB_ERR_INVALID, "proving key was built for different Params");
+    const Context& ctx = params.context();
+    ctx.check(tb_dev_prove_batch(ctx.get(), pk.get(), n, d_advice, d_instance, instance_len.empty() ? nullptr : instance_len.data(), rng_seed.data(),
+                                 first_proof_index, d_proofs, proof_stride, d_status));
+  }
+
   // MockProver::run(k, circuit, instance).verify() for n witnesses, without proving (verify_transparently).  `circuits` and
   // `instances` as in create_batch.  `seed` must be unpredictable to whoever wrote the witnesses: gates and lookups are tested
   // through random combinations drawn from it (a failure escapes with probability about (constraints + lookup width) / p).

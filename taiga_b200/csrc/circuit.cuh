@@ -19,7 +19,13 @@ inline PolyId column_poly(const tb_column& col) { return {col.kind == TB_COL_ADV
 // Scratch of one (context, batch size) pair: device blocks in request order and the small tables uploaded on first use.
 // A tb_pk may be shared by several contexts (= host threads); each gets its own workspace, and a second thread entering
 // with the SAME context and batch size while a call is in flight is refused (TB_ERR_INVALID) instead of corrupting it.
-struct ProveWs { std::vector<DevMem<uint8_t>> blocks, tables; std::vector<std::vector<uint8_t>> table_bytes; std::atomic<int> busy{0}; };
+// `busy` covers the host call only.  A device call (tb_dev_prove_batch) returns with its work still queued: `idle` is recorded
+// on the context's stream after that work, and the workspace is not freed before it has completed.  Two calls on the same
+// context need no more than that (stream order keeps them apart); a host call waits for its stream, so `idle` has then passed.
+struct ProveWs {
+  std::vector<DevMem<uint8_t>> blocks, tables; std::vector<std::vector<uint8_t>> table_bytes; std::atomic<int> busy{0};
+  Ctx::Event idle;
+};
 
 // Everything the description fixes, built once by shape_build: sizes, domain constants, the compiled programs and the
 // order of the proof's elements.  Host memory only and nothing per row, so a verifying key costs kilobytes.
@@ -69,6 +75,10 @@ struct Circuit : Shape {
   mutable DevMem<uint32_t> sig_next;
   mutable DevMem<QInstr> single_code; mutable DevMem<int2> single_table; mutable int single_nregs = 0; mutable bool check_ready = false;
   explicit Circuit(Shape&& s) : Shape(std::move(s)) {}
+  // tb_pk_free: the workspaces' device calls may still be queued; their memory is freed only after each has completed
+  ~Circuit() {
+    for (auto& w : ws) try { w.second->idle.wait(); } catch (const CudaError&) {}
+  }
   // the workspace of (context, batch size), marked busy; nullptr if a call is already using it.  Claiming under the lock
   // lets release_idle() free every workspace that is not marked.  Checks (`check`) keep workspaces apart from proofs: their
   // buffers differ, and sharing would reallocate on every switch between the two.
@@ -80,12 +90,14 @@ struct Circuit : Shape {
   }
   // Out of device memory on `device` (the calling context's): frees the workspaces no call is using (other batch sizes, other
   // contexts) and what the stream-ordered pool keeps cached, so that scratch kept for earlier calls does not make a new batch size fail.
+  // A workspace whose last device call is still queued or running is kept: `busy` is cleared only after `idle` is recorded, so
+  // under the lock a workspace that is not busy has its last call's mark in `idle`.
   void release_idle(int device) const {
     TB_CUDA(cudaDeviceSynchronize());
     {
       std::lock_guard<std::mutex> lk(mu);
       for (auto it = ws.begin(); it != ws.end();) {
-        if (it->second->busy.load() != 0) { ++it; continue; }
+        if (it->second->busy.load() != 0 || !it->second->idle.done()) { ++it; continue; }
         it = ws.erase(it);
       }
     }

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <initializer_list>
 #include <stdexcept>
 #include <string>
 #include <map>
@@ -115,6 +116,28 @@ struct Ctx {
     if (!event_pool.empty()) { e = event_pool.back(); event_pool.pop_back(); return e; }
     TB_CUDA(cudaEventCreate(&e)); return e;
   }
+  // An event owned by whoever holds it, not by a context: it may outlive the context whose stream recorded it (a proving
+  // key's workspace keeps the mark of its last device call).  Created on first record; destroying it with work still
+  // pending is allowed (the driver releases it when the work is done).
+  struct Event {
+    cudaEvent_t e = nullptr;
+    Event() {}
+    Event(const Event&) = delete; Event& operator=(const Event&) = delete;
+    ~Event() { if (e) cudaEventDestroy(e); }
+    void record(cudaStream_t s) {
+      if (!e) TB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      TB_CUDA(cudaEventRecord(e, s));
+    }
+    // true once the stream has passed the last record (and for an event never recorded)
+    bool done() const {
+      if (!e) return true;
+      cudaError_t r = cudaEventQuery(e);
+      if (r == cudaErrorNotReady) return false;
+      TB_CUDA(r);
+      return true;
+    }
+    void wait() const { if (e) TB_CUDA(cudaEventSynchronize(e)); }
+  };
 
   template <class T> T* alloc(size_t count) {
     void* p = nullptr;
@@ -173,6 +196,18 @@ template <class T> struct DevBuf {
   void upload(const void* host, size_t count) { TB_CUDA(cudaMemcpyAsync(p, host, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream)); }
   void download(void* host, size_t count) const { TB_CUDA(cudaMemcpyAsync(host, p, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream)); }
 };
+
+// Refuses (TB_ERR_INVALID) a pointer that is not device memory of the context's device; nullptr entries are skipped.  The
+// entry points that take device buffers (the device prover and verifier) check them with it before they enqueue anything.
+inline void require_device_memory(const Ctx& ctx, std::initializer_list<const void*> ptrs, const char* what) {
+  for (const void* p : ptrs) {
+    if (!p) continue;
+    cudaPointerAttributes a;
+    TB_CUDA(cudaPointerGetAttributes(&a, p));
+    TB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx.device,
+               std::string(what) + ": a buffer is not device memory of the context's device");
+  }
+}
 
 template <class F> inline FieldTables<F>& field_tables(Ctx* c);
 template <> inline FieldTables<Fp>& field_tables<Fp>(Ctx* c) { return c->tw_fp; }

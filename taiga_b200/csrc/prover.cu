@@ -135,6 +135,35 @@ __global__ void fill_const_kernel(Fp* v, size_t count, Fp val) {
   if (i < count) st_fe(v + i, val);
 }
 
+// The tail of a device call (tb_dev_prove_batch), one block per proof: status[b] = 1 + the lowest lookup whose input is missing
+// from its table (derr [B][L]), else TB_PROVE_INTERNAL if the transcript reports an error or a length other than proof_len, else
+// TB_PROVED; then the record out + b * stride is the transcript's bytes (status TB_PROVED) or zeros.  16-byte stores where the
+// record is 16-byte aligned, byte stores otherwise; nothing outside the record is written.
+__global__ void prove_emit_kernel(const uint32_t* __restrict__ derr, int L, const TrState* __restrict__ st, const uint8_t* __restrict__ proofs,
+                                  uint32_t proof_len, uint8_t* out, size_t stride, uint32_t* status) {
+  __shared__ uint32_t s_status;
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    uint32_t s = TB_PROVED;
+    for (int l = L - 1; l >= 0; --l)
+      if (derr[(size_t)b * L + l]) s = 1u + (uint32_t)l;
+    if (s == TB_PROVED && (st[b].error || st[b].proof_len != proof_len)) s = TB_PROVE_INTERNAL;
+    status[b] = s;
+    s_status = s;
+  }
+  __syncthreads();
+  const bool keep = s_status == TB_PROVED;
+  const uint8_t* src = proofs + (size_t)b * proof_len;   // 32-byte aligned: proof_len is a multiple of 32
+  uint8_t* dst = out + (size_t)b * stride;
+  if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+    const uint4 zero = make_uint4(0, 0, 0, 0);
+    for (uint32_t i = threadIdx.x; i < proof_len / 16; i += blockDim.x)
+      reinterpret_cast<uint4*>(dst)[i] = keep ? reinterpret_cast<const uint4*>(src)[i] : zero;
+  } else {
+    for (uint32_t i = threadIdx.x; i < proof_len; i += blockDim.x) dst[i] = keep ? src[i] : 0;
+  }
+}
+
 // ---------------------------------------------------------------- the prover
 struct VarAlloc {
   int next = 0;
@@ -176,8 +205,12 @@ void upload_witness(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice, co
     prf_fill(ctx, seed, proof0, rows_tag, (uint32_t)(c * (bf + 1)), adv_vals + (size_t)c * n + C.usable, (long long)na * n, 1, bf + 1, B);
 }
 
-static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice_host, const uint8_t* instance_host, const uint32_t* instance_len,
-                        const uint8_t* seed, uint32_t proof0, uint8_t* proofs_out, size_t proof_stride) {
+// B proofs of circuit C.  `advice` and `instance` may be host or device pointers.  Where the proofs go is the only branch, after
+// the last transcript write: `on_device` false, proofs_out is host memory, the call waits for the device and throws for a failing
+// proof (tb_prove_batch); `on_device` true, proofs_out and status_out are device memory, prove_emit_kernel writes a status per
+// proof and its record, and the call returns without waiting (tb_dev_prove_batch).
+static void prove_batch(Ctx* ctx, bool on_device, const Circuit& C, int B, const uint8_t* advice, const uint8_t* instance, const uint32_t* instance_len,
+                        const uint8_t* seed, uint32_t proof0, uint8_t* proofs_out, size_t proof_stride, uint32_t* status_out) {
   const Srs& srs = *C.srs;
   const size_t n = C.n; const long long nn = (long long)n; const int k = (int)C.k; const int na = C.na, ni = C.ni, L = C.L, nsets = C.nsets, P = C.P, bf = C.bf;
   const int ni1 = std::max(1, ni), L1 = std::max(1, L), ns1 = std::max(1, nsets);
@@ -191,7 +224,15 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   ProveWs* claimed = C.claim_workspace(ctx, B);
   TB_REQUIRE(claimed != nullptr, "this proving key / context / batch size is already proving on another thread (a tb_ctx is bound to one thread)");
   ProveWs& pws = *claimed;
-  struct BusyGuard { std::atomic<int>& f; ~BusyGuard() { f.store(0); } } guard{pws.busy};
+  // runs after every other local's clean-up (the stream-ordered frees included): a device call marks the end of its queued
+  // work in `idle` before the workspace can be taken or released, on error paths too
+  struct BusyGuard {
+    ProveWs& w; cudaStream_t st; bool on_device;
+    ~BusyGuard() {
+      if (on_device) try { w.idle.record(st); } catch (const CudaError&) {}
+      w.busy.store(0);
+    }
+  } guard{pws, st, on_device};
   WsAlloc ws{ctx, C, pws.blocks};
   std::vector<DevMem<uint8_t>>& tables = pws.tables;
   size_t table_cur = 0;
@@ -256,7 +297,7 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   WBuf<Fp> adv_vals; adv_vals.p = first.get() + (size_t)B * ni * n; adv_vals.n = (size_t)B * na * n; adv_vals.ctx = ctx;
   Fp* const inst_polys = polys.get() + (size_t)O_INST * n;
   Fp* const adv_polys = polys.get() + (size_t)O_ADV * n;
-  upload_witness(ctx, C, B, advice_host, instance_host, instance_len, seed, proof0, R_ADVICE_ROWS, inst_vals.get(), adv_vals.get());
+  upload_witness(ctx, C, B, advice, instance, instance_len, seed, proof0, R_ADVICE_ROWS, inst_vals.get(), adv_vals.get());
   if (ni) launch(ctx, fill_const_kernel, (B * ni + 63) / 64, 64, 0, blinds.get(), (size_t)B * ni, Fp::one());
   // ---- advice columns: commit, iNTT
   prf_fill(ctx, seed, proof0, R_ADVICE_BLIND, 0, VP(V_ADV_BLIND), NV, 1, na, B);
@@ -575,7 +616,12 @@ static void prove_batch(Ctx* ctx, const Circuit& C, int B, const uint8_t* advice
   tr.scalars(VP(V_C), NV, 1, true);
   tr.scalars(VP(V_F), NV, 1, true);
 
-  // ---- download (the only host synchronisation of the call)
+  // ---- device memory: a status per proof and its record, in stream order; no host synchronisation
+  if (on_device) {
+    launch(ctx, prove_emit_kernel, B, 128, 0, derr.get(), L, tr.states.get(), tr.proofs.get(), C.proof_len, proofs_out, proof_stride, status_out);
+    return;
+  }
+  // ---- host memory: download (the only host synchronisation of the call)
   std::vector<TrState> hst(B);
   std::vector<uint32_t> herr((size_t)B * L1, 0);
   TB_CUDA(cudaMemcpyAsync(hst.data(), tr.states.get(), (size_t)B * sizeof(TrState), cudaMemcpyDeviceToHost, st));
@@ -616,7 +662,22 @@ tb_status tb_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const 
   TB_REQUIRE(C && n_proofs >= 1 && advice && seed && proofs_out && proof_stride >= C->proof_len && (C->ni == 0 || (instance && instance_len)), "tb_prove_batch arguments");
   TB_REQUIRE((uint64_t)n_proofs * std::max<uint32_t>(C->na, C->pieces) <= 65535, "batch too large for one call");
   TB_CUDA(cudaSetDevice(ctx->c.device));
-  prove_batch(&ctx->c, *C, (int)n_proofs, advice, instance, instance_len, seed, first_proof_index, proofs_out, proof_stride);
+  prove_batch(&ctx->c, false, *C, (int)n_proofs, advice, instance, instance_len, seed, first_proof_index, proofs_out, proof_stride, nullptr);
+  TB_API_END(ctx)
+}
+
+tb_status tb_dev_prove_batch(tb_ctx* ctx, const tb_pk* pk, uint32_t n_proofs, const void* d_advice, const void* d_instance, const uint32_t* instance_len,
+                             const uint8_t seed[32], uint32_t first_proof_index, void* d_proofs_out, size_t proof_stride, uint32_t* d_status_out) {
+  TB_API_BEGIN(ctx)
+  const Circuit* C = reinterpret_cast<const Circuit*>(pk);
+  TB_REQUIRE(C && n_proofs >= 1 && d_advice && seed && d_proofs_out && d_status_out && proof_stride >= C->proof_len && (C->ni == 0 || (d_instance && instance_len)),
+             "tb_dev_prove_batch arguments");
+  TB_REQUIRE((uint64_t)n_proofs * std::max<uint32_t>(C->na, C->pieces) <= 65535, "batch too large for one call");
+  instance_total(*C, instance_len);
+  TB_CUDA(cudaSetDevice(ctx->c.device));
+  require_device_memory(ctx->c, {d_advice, d_proofs_out, d_status_out, C->ni ? d_instance : nullptr}, "tb_dev_prove_batch");
+  prove_batch(&ctx->c, true, *C, (int)n_proofs, static_cast<const uint8_t*>(d_advice), static_cast<const uint8_t*>(d_instance), instance_len, seed,
+              first_proof_index, static_cast<uint8_t*>(d_proofs_out), proof_stride, d_status_out);
   TB_API_END(ctx)
 }
 

@@ -12,7 +12,6 @@
 #define TB_NOINLINE_MUL 1
 #include <algorithm>
 #include <cstdlib>
-#include <initializer_list>
 #include "capi_internal.cuh"
 #include "circuit.cuh"
 #include "replay.cuh"
@@ -469,17 +468,6 @@ static std::vector<Aff<Fq>> parse_commitments(const uint8_t* b, size_t cnt, cons
     out[i] = p;
   }
   return out;
-}
-
-// Refuses (TB_ERR_INVALID) a pointer that is not device memory of the context's device; nullptr entries are skipped
-static void require_device_memory(const Ctx& ctx, std::initializer_list<const void*> ptrs, const char* what) {
-  for (const void* p : ptrs) {
-    if (!p) continue;
-    cudaPointerAttributes a;
-    TB_CUDA(cudaPointerGetAttributes(&a, p));
-    TB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx.device,
-               std::string(what) + ": a buffer is not device memory of the context's device");
-  }
 }
 
 // Refuses (TB_ERR_INVALID, "<what> arguments") a verifier call of no proofs or more than 4096, without proofs, with rows

@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(_HERE, "libtaiga_b200.so")
 TB_FP, TB_FQ = 0, 1
 TB_VESTA, TB_PALLAS = 0, 1
 TB_OK, TB_ERR_INVALID, TB_ERR_CUDA, TB_ERR_CONSTRAINT, TB_ERR_INTERNAL = 0, 1, 2, 3, 4
+# status of one proof of tb_dev_prove_batch: proved, 1 + l (an input of lookup l is not in its table), or an internal error
+# (0xFFFFFFFF, which reads as -1 in the int32 status tensors of ProvingKey.prove_batch_dev)
+TB_PROVED, TB_PROVE_INTERNAL = 0, 0xFFFFFFFF
 
 
 class TaigaB200Error(RuntimeError):
@@ -59,6 +62,7 @@ _SIGS = {
     "tb_pk_proof_len": (_sz, [_vp]),
     "tb_pk_commitments": (_i, [_vp, _vp, _vp, _vp]),
     "tb_prove_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _sz]),
+    "tb_dev_prove_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _sz, _vp]),
     "tb_verify_batch": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _sz, _sz, _vp]),
     "tb_decompress": (_i, [_vp, _sz, _vp, _vp, _vp]),
     "tb_vk_load": (_i, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
@@ -313,6 +317,25 @@ class ProvingKey:
                                            _ptr(out), self.proof_len))
         return [out[b].tobytes() for b in range(B)]
 
+    def prove_batch_dev(self, advice, instance, instance_len, seed, proofs, status, first_proof_index=0, ctx=None):
+        """prove_batch into device memory, enqueued on the context's stream without waiting (tb_dev_prove_batch).  `advice` a
+        contiguous CUDA uint8 tensor of B witnesses (B * num_advice * n * 32 bytes), `instance` a contiguous CUDA uint8 tensor of
+        B * sum(instance_len) * 32 bytes (or None without instance columns), `proofs` a CUDA uint8 tensor [B, >= proof_len] (one
+        record per row, any row stride), `status` a CUDA int32 tensor of B statuses: TB_PROVED, 1 + l for a missing input of
+        lookup l, or TB_PROVE_INTERNAL (reads as -1).  A record whose status is not TB_PROVED is all zeros.  The context's
+        stream first waits for torch's current stream, and the tensors are kept from reuse until it has run the call (torch
+        records an event on the context's stream when it frees them: free them before closing the context)."""
+        ctx = ctx or self.ctx
+        kd = self.keydata
+        assert advice.is_cuda and advice.dtype.itemsize == 1 and advice.is_contiguous()
+        assert status.is_cuda and str(status.dtype) == "torch.int32" and status.is_contiguous() and status.numel() >= proofs.shape[0]
+        B, inst, lens, addr, stride, plen = _dev_args(ctx, instance, instance_len, proofs, None, advice, status)
+        assert plen >= self.proof_len and advice.numel() == B * kd.cs.num_advice * kd.n * 32
+        seed = _u8(np.frombuffer(bytes(seed), np.uint8))
+        assert seed.size == 32
+        ctx._check(ctx._lib.tb_dev_prove_batch(ctx._h, self._h, B, _vp(advice.data_ptr()), inst, _ptr(lens), _ptr(seed), first_proof_index,
+                                               addr, stride, _vp(status.data_ptr())))
+
     def verify_batch(self, instance, instance_len, proofs, ctx=None):
         """Proof::verify for a batch: proofs = list of byte strings; returns a list of booleans."""
         return _verify_batch(ctx or self.ctx, "tb_verify_batch", self._h, instance, instance_len, proofs)
@@ -384,11 +407,13 @@ def _verify_batch(ctx, fn, h, instance, instance_len, proofs):
 
 
 def _dev_args(ctx, instance, instance_len, proofs, proof_len, *tensors):
-    """(n_proofs, instance, instance_len, proofs, proof_stride, proof_len) of a verifier call on device memory: `proofs` a
-    CUDA uint8 tensor of B proof records, one per row (rows may be padded or be views with any row stride; proof_len defaults
-    to the row length), `instance` a contiguous CUDA uint8 tensor or None.  Orders the context's stream after the work torch
-    has enqueued on its current stream (what made the tensors the call reads), and marks `proofs`, `instance` and `tensors` as
-    used on the context's stream, so that torch's allocator does not hand their memory out again before the call has run there."""
+    """(n_proofs, instance, instance_len, proofs, proof_stride, proof_len) of a prover or verifier call on device memory:
+    `proofs` a CUDA uint8 tensor of B proof records, one per row (rows may be padded or be views with any row stride;
+    proof_len defaults to the row length), read by the verifier and written by the prover; `instance` a contiguous CUDA uint8
+    tensor or None; `tensors` the call's other device buffers (verdicts; advice and statuses).  Orders the context's stream
+    after the work torch has enqueued on its current stream (what made or last read the tensors), and marks `proofs`,
+    `instance` and `tensors` as used on the context's stream, so that torch's allocator does not hand their memory out again
+    before the call has run there."""
     import torch
     assert proofs.is_cuda and proofs.dtype.itemsize == 1 and proofs.dim() == 2 and proofs.stride(1) == 1
     assert instance is None or (instance.is_cuda and instance.dtype.itemsize == 1 and instance.is_contiguous())

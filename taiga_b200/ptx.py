@@ -14,6 +14,7 @@ The circuits are the Taiga-shaped ones of circuits_taiga.py (the real ones need 
 synthesis happens on the host before the call, exactly as `Circuit::synthesize` does in the reference; it is not part
 of the proving hot path and not part of any timed region.
 """
+import itertools
 import os
 import threading
 
@@ -84,14 +85,7 @@ class ProverService:
         the GPU from one stream per circuit; single partial transactions want two, to overlap their latency-bound phases)."""
         c_adv = wit["c_adv"] if c_adv is None else c_adv
         v_adv = wit["v_adv"] if v_adv is None else v_adv
-        jobs = []   # (result slot, worker, first proof, last proof, ...)
-        for kind, workers, adv, inst, lens, index0 in (("c", self.c_workers, c_adv, wit["c_inst"], wit["c_len"], 0),
-                                                       ("v", self.v_workers, v_adv, wit["v_inst"], wit["v_len"], 1 << 20)):
-            total = len(inst)
-            nw = min(len(workers) if not workers_per_circuit else min(len(workers), workers_per_circuit), total)
-            for w in range(nw):
-                lo, hi = total * w // nw, total * (w + 1) // nw
-                jobs.append((kind, lo, hi, workers[w], adv, inst, lens, index0))
+        jobs = self._jobs(wit, c_adv, v_adv, workers_per_circuit)
         results, errors = {}, []
 
         def run(job):
@@ -116,6 +110,57 @@ class ProverService:
         for (kind, lo) in sorted(results):
             out[kind] += results[(kind, lo)]
         return out["c"], out["v"]
+
+    def build_ptx_batch_dev(self, wit, seed, c_adv=None, v_adv=None, max_batch=64, workers_per_circuit=None):
+        """build_ptx_batch into device memory from the calling thread: every chunk of every worker is enqueued on that worker's
+        context (ProvingKey.prove_batch_dev) and the call returns without waiting.  Returns (compliance proofs, vp proofs,
+        compliance statuses, vp statuses) as CUDA tensors ([N, proof_len] uint8 and [N] int32, TB_PROVED for a written proof),
+        ordered on torch's current stream after the workers: torch work enqueued after the call reads finished proofs.  The
+        proofs are the bytes build_ptx_batch returns for the same arguments.  c_adv / v_adv: the advice as CUDA tensors
+        (default: wit's host arrays, copied to the device first)."""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+
+        def on_device(a):
+            return a if hasattr(a, "is_cuda") and a.is_cuda else torch.from_numpy(np.ascontiguousarray(a, dtype=np.uint8)).to(dev)
+        c_adv = on_device(wit["c_adv"] if c_adv is None else c_adv)
+        v_adv = on_device(wit["v_adv"] if v_adv is None else v_adv)
+        out = {}
+        for kind, pk in (("c", self.pk_c), ("v", self.pk_v)):
+            n = len(wit[kind + "_inst"])
+            out[kind] = (torch.zeros((n, pk.proof_len), dtype=torch.uint8, device=dev), torch.zeros(n, dtype=torch.int32, device=dev),
+                         on_device(wit[kind + "_inst"]).reshape(n, -1))
+        jobs = self._jobs(wit, c_adv, v_adv, workers_per_circuit)
+        calls = [[(kind, ctx, pk, adv, lens, index0, s, e) for s, e in _chunks(lo, hi, max_batch)]
+                 for kind, lo, hi, (ctx, pk), adv, _, lens, index0 in jobs]
+        # the workers' calls in turn: a call can hold the thread until its stream has run most of it (the driver queues only
+        # so many launches), so the next call goes to another worker's stream
+        for turn in itertools.zip_longest(*calls):
+            for kind, ctx, pk, adv, lens, index0, s, e in (c for c in turn if c is not None):
+                proofs, status, inst = out[kind]
+                flat = adv.reshape(len(inst), -1)
+                pk.prove_batch_dev(flat[s:e], inst[s:e], lens, seed, proofs[s:e], status[s:e], first_proof_index=index0 + s, ctx=ctx)
+        used = [w[0] for _, _, _, w, _, _, _, _ in jobs]
+        cur = torch.cuda.current_stream(dev)
+        for ctx in used:   # torch's stream goes on after every worker's last call
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.ExternalStream(ctx.stream, device=dev))
+            cur.wait_event(ev)
+        return out["c"][0], out["v"][0], out["c"][1], out["v"][1]
+
+    def _jobs(self, wit, c_adv, v_adv, workers_per_circuit=None):
+        """The split of a bundle among the workers, shared by build_ptx_batch and build_ptx_batch_dev: per circuit, up to
+        workers_per_circuit of its (context, key) pairs take consecutive ranges [lo, hi) of its proofs.  Proof i of a circuit
+        gets the proof index index0 + i, wherever it is proved.  Returns [(kind, lo, hi, worker, advice, instance, lens, index0)]."""
+        jobs = []
+        for kind, workers, adv, inst, lens, index0 in (("c", self.c_workers, c_adv, wit["c_inst"], wit["c_len"], 0),
+                                                       ("v", self.v_workers, v_adv, wit["v_inst"], wit["v_len"], 1 << 20)):
+            total = len(inst)
+            nw = min(len(workers) if not workers_per_circuit else min(len(workers), workers_per_circuit), total)
+            for w in range(nw):
+                lo, hi = total * w // nw, total * (w + 1) // nw
+                jobs.append((kind, lo, hi, workers[w], adv, inst, lens, index0))
+        return jobs
 
     def check_ptx_batch(self, wit, seed, max_failures=16):
         """The batched verify_transparently: MockProver::run(15, ..).verify() of all 2P Compliance and 4P VP witnesses of
@@ -142,7 +187,9 @@ class ProverService:
         """The proof part of ShieldedPartialTxBundle::execute (shielded_ptx.rs:137-153) for the partial transactions of
         `wit` (what synthesize_ptx returns): every Compliance and VP proof goes into one BatchVerifier, finalized once.  `seed`
         (32 bytes) must be unpredictable to whoever made the proofs.  Returns (all accepted, [verdict per partial transaction]);
-        when the batch is rejected, each circuit's proofs are verified one by one to name the failing partial transactions."""
+        when the batch is rejected, each circuit's proofs are verified one by one to name the failing partial transactions.
+        c_proofs / v_proofs: lists of byte strings, or CUDA tensors of one proof per row (what build_ptx_batch_dev returns),
+        which are read where they are."""
         n_ptx = len(wit["c_inst"]) // COMPLIANCE_PER_PTX
         assert len(c_proofs) == COMPLIANCE_PER_PTX * n_ptx and len(v_proofs) == VP_PER_PTX * n_ptx
         circuits = [(vk, proofs, inst, lens, per) for vk, proofs, inst, lens, per in
@@ -150,8 +197,14 @@ class ProverService:
                         (COMPLIANCE_PER_PTX, VP_PER_PTX))]
         import torch
         dev = torch.device("cuda", self.srs.ctx.device)
-        # the bundle's proof records and instances go to the device once; the replay, the MSMs and the checks run there
-        on_dev = [(vk, torch.from_numpy(np.frombuffer(b"".join(proofs), np.uint8).reshape(len(proofs), -1).copy()).to(dev),
+
+        def proofs_on_device(proofs):
+            if hasattr(proofs, "is_cuda") and proofs.is_cuda:
+                return proofs
+            return torch.from_numpy(np.frombuffer(b"".join(proofs), np.uint8).reshape(len(proofs), -1).copy()).to(dev)
+        # the bundle's proof records and instances go to the device once (unless already there); the replay, the MSMs and the
+        # checks run there
+        on_dev = [(vk, proofs_on_device(proofs),
                    torch.from_numpy(np.ascontiguousarray(inst, dtype=np.uint8).reshape(len(proofs), -1).copy()).to(dev), lens, per)
                   for vk, proofs, inst, lens, per in circuits]
         bv = lib.BatchVerifier(self.srs, seed)
@@ -202,14 +255,18 @@ class ProverService:
         per = kd.cs.num_advice * kd.n * 32
         total = len(inst)
         out = []
-        for s in range(lo, hi, max_batch):
-            e = min(hi, s + max_batch)
+        for s, e in _chunks(lo, hi, max_batch):
             if hasattr(adv, "data_ptr"):  # torch tensor (pinned host or device)
                 chunk = _TensorSlice(adv, s * per, (e - s) * per)
             else:
                 chunk = adv.reshape(total, -1)[s:e]
             out += pk.prove_batch_raw(chunk, e - s, inst[s:e], lens, seed, index0 + s, ctx=ctx)
         return out
+
+
+def _chunks(lo, hi, max_batch):
+    """the calls [s, e) of a worker's range [lo, hi): at most max_batch proofs each, the first proof of each at index0 + s"""
+    return [(s, min(hi, s + max_batch)) for s in range(lo, hi, max_batch)]
 
 
 _SYNTH = None
